@@ -44,7 +44,7 @@ SYMBOLS = [
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
-TUNE_GAP_MODE, TUNE_CTAS_PER_SM, TUNE_HOST_THREADS = 0, 1, 2
+TUNE_GAP_MODE, TUNE_CTAS_PER_SM, TUNE_HOST_THREADS, TUNE_AGG_PIPELINE = 0, 1, 2, 3
 
 
 class PackedSetC(C.Structure):

@@ -87,12 +87,12 @@ constexpr size_t   kAggRingSmem   = kRingBytes + kRingTail;       // blocks neve
 // window offset = the driver's reserved bytes (1 KB on sm_90), so the pad depends on the kernel's static size -- the host
 // computes it (agg_dyn_smem) and the kernel re-derives the position from the real address.
 constexpr uint32_t kLiveAlign     = 8192u;
-__host__ inline size_t agg_dyn_smem(size_t static_bytes, size_t reserved_bytes)
+__host__ inline size_t agg_dyn_smem(size_t static_bytes, size_t reserved_bytes, size_t ring_bytes = kAggRingSmem)
 {
     const size_t start = reserved_bytes + static_bytes;                   // window offset of the dynamic region (before its own alignment)
     const size_t start_al = (start + 127) & ~(size_t)127;
     const size_t k_at = (start_al + kLiveAlign - 1) & ~(size_t)(kLiveAlign - 1);
-    return (k_at - start) + kLiveAlign + kAggRingSmem + 128;
+    return (k_at - start) + kLiveAlign + ring_bytes + 128;
 }
 // FLAT consumer: the ring is cut into one private slot per warp; warp w streams chunks w, w+16, ... of the window through
 // its own slot and its own mbarrier -- no cross-warp hand-off, the per-chunk overhead is paid once per slot, not 16 times
@@ -186,6 +186,18 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 __device__ __forceinline__ void fence_proxy_async()
 {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar, uint32_t count = 1u)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory");
+}
+// Block barrier over the kAggThreads threads that compute a column: the whole CTA (__syncthreads) in agg_kernel, named barrier 1
+// over the consumer warps in agg_pipe_kernel (PIPE), whose producer warp never joins it.
+template <bool PIPE>
+__device__ __forceinline__ void agg_sync()
+{
+    if (PIPE) asm volatile("bar.sync 1, %0;" :: "n"(kAggThreads) : "memory");
+    else      __syncthreads();
 }
 
 // raw 32-bit shared-window addresses keep the scatter loop free of generic->shared conversions
@@ -483,11 +495,11 @@ __host__ __device__ __forceinline__ uint32_t binop_rule(uint32_t op, uint32_t ka
     }
 }
 
-// Epilogue shared by agg_kernel and finalize_blocks_kernel: R = this thread's 4 words of the result block.
+// Epilogue shared by agg_kernel, agg_pipe_kernel and finalize_blocks_kernel: R = this thread's 4 words of the result block.
 // state: 0 = nothing stored, 1 = FULL, 2 = computed block.  Fuses bit_block_count, calc_block_digest0,
 // bit_block_calc_change, the opt_copy_bit_block classification and its bit_to_gap branch
 // (src/bmfunc.h:5808,1239,6040,5540; src/bmblocks.h:1355-1409).
-template <bool EMPTY_DIGEST_IS_NULL>
+template <bool EMPTY_DIGEST_IS_NULL, bool PIPE = false>
 __device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, uint32_t colx, uint32_t grp, uint4 R, int state,
                                              uint32_t* K, uint32_t* s_pc, uint32_t* s_tr, uint32_t* s_dg, uint32_t rule = 0u)
 {
@@ -501,7 +513,7 @@ __device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, u
 #pragma unroll
     for (int q = 0; q < 4; ++q) if ((bal >> (8 * q)) & 0xffu) dg4 |= (1u << q);
     uint32_t pc = warp_sum(popc4(R));
-    __syncthreads();
+    agg_sync<PIPE>();
     // x has a bit at every position p whose successor differs (bit_block_calc_change src/bmfunc.h:6040 counts
     // them; bit_block_to_gap src/bmfunc.h:5540 emits them as run ends); bit 65535 has no successor
     const uint32_t nxt = (tid + 1 < kAggThreads) ? (K[4 * tid + 4] & 1u) : (R.w >> 31);
@@ -513,7 +525,7 @@ __device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, u
     for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
     if (lane == 31) s_tr[warp] = inc;
     if (lane == 0) { s_pc[warp] = pc; s_dg[warp] = dg4; }
-    __syncthreads();
+    agg_sync<PIPE>();
     uint32_t tpc = 0, ttr = 0, woff = 0; uint64_t dg = 0;
 #pragma unroll
     for (int w = 0; w < kAggWarps; ++w) {
@@ -578,6 +590,17 @@ __device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, u
         p.kind[col]   = (uint8_t)kd;
         if (tpc) atomicAdd(p.total + grp, (unsigned long long)tpc);
     }
+}
+
+// AND / AND-SUB result state (0 = NULL, 1 = FULL, 2 = computed): an AND-group NULL block, an empty AND group or a SUB-group FULL
+// block empties the column; an AND group of FULL blocks only, with no SUB group (AND-SUB), fills it
+template <int OP>
+__device__ __forceinline__ int and_state(uint32_t flags, uint32_t tot_bit0, uint32_t tot_gap0, uint32_t n0, uint32_t n1)
+{
+    if ((flags & kFlNull0) || n0 == 0) return 0;
+    if (flags & kFlFull1) return 0;
+    if (tot_bit0 + tot_gap0 == 0 && (OP == BMB200_OP_AND || n1 == 0)) return 1;
+    return 2;
 }
 
 template <int OP>
@@ -991,16 +1014,258 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
             const uint32_t inv = (tot_full0 & 1u) ? 0xffffffffu : 0u;
             R = make_uint4(k4.x ^ inv, k4.y ^ inv, k4.z ^ inv, k4.w ^ inv);
         } else {
-            if ((flags & kFlNull0) || n0 == 0) state = 0;
-            else if (flags & kFlFull1) state = 0;
-            else if (tot_bit0 + tot_gap0 == 0 && (OP == BMB200_OP_AND || n1 == 0)) state = 1;
-            else state = 2;
+            state = and_state<OP>(flags, tot_bit0, tot_gap0, n0, n1);
             R = k4;
         }
         if (state == 0) R = make_uint4(0u, 0u, 0u, 0u);
         if (state == 1) R = make_uint4(~0u, ~0u, ~0u, ~0u);
 
         finish_block<OP != BMB200_OP_OR>(p, col, colx, grp, R, state, K, s_pc, s_tr, s_dg, rule);
+    }
+}
+
+// ---- whole-set AND-SUB: a producer warp streams every column through a shared-memory stage ring ----
+//
+// When the argument is ONE AND-SUB group whose group0 + group1 name every vector of the set exactly once,
+// every block of column nb is needed: its bit-blocks are the contiguous run bit_pool[bit_base[nb] .. bit_base[nb+1]) and its GAP
+// blocks the contiguous units gap_pool[gap_base[nb] .. gap_base[nb+1]).  No member list has to be resolved before the bytes can be
+// requested, so one producer warp streams columns back to back with cp.async.bulk into a ring of 8 KB stages (full / empty mbarrier
+// per stage) and HBM keeps ~kPipeStages x 8 KB per SM in flight across column boundaries, while 16 consumer warps classify the
+// column from its descriptor row, fold the staged bit-blocks (stage j = bit-block j of the segment) and sweep the staged GAP segment
+// in FLAT form.  A column whose GAP blocks are not all FLAT SUB-group blocks (raw GAP form, GAP blocks in the AND group) releases
+// its GAP stages unread and applies its GAP blocks straight from global memory.
+// Protocol (no wait can outlive the producer): the producer claims a column only when a queue slot is free, publishes (item, #bit
+// stages, GAP bytes, first stage) and then issues all of the column's stages in order, each after its empty barrier; after the last
+// column it publishes an end marker.  Consumers read every queue entry, wait for exactly the stages the entry announces and release
+// each of them exactly once (bit stage: every warp arrives; GAP stage: its one reader arrives for all 16).
+// Parity waits are only sound when the waiter has seen the stage's previous fill complete.  Bit stages are waited for by every
+// warp in order; GAP stage g goes to warp g % 16, so with a ring of a multiple of 16 stages the previous fill of each stage a warp
+// waits for was one of its own GAP stages, or a bit stage / an earlier column that every warp has finished.
+constexpr int      kPipeStages  = 16;                      // 128 KB of stages
+constexpr uint32_t kPipeStage   = 8192u;
+constexpr int      kPipeQueue   = 2;                       // columns claimed ahead of the consumers (more would unbalance the tail)
+constexpr uint32_t kPipeMaxVec  = 4096u;                   // role table size: larger sets take agg_kernel
+constexpr int      kPipePerThr  = (int)kPipeMaxVec / kAggThreads;
+constexpr uint32_t kPipeMaxAndGap = 64u;                   // AND-group GAP blocks per column the FLAT path takes (more: in-place reads)
+constexpr uint32_t kPipeThreads = kAggThreads + 32u;       // 16 consumer warps + 1 producer warp
+constexpr size_t   kPipeRingSmem = (size_t)kPipeStages * kPipeStage;
+static_assert(kPipeStages % kAggWarps == 0, "GAP stage g is consumed by warp g % 16: the ring must hold a multiple of 16 stages");
+
+// *bad |= 1 when a GAP block of the set is not in the BMB200_DESC_GAP_FLAT form (agg_pipe_kernel sweeps SUB-group blocks as FLAT pairs)
+__global__ void desc_flat_check_kernel(const uint32_t* __restrict__ desc, size_t n, uint32_t* bad)
+{
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t d = desc[i];
+        if ((d & 3u) == BMB200_BLK_GAP && !(d & BMB200_DESC_GAP_FLAT)) { atomicOr(bad, 1u); return; }
+    }
+}
+
+__global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggParams p)
+{
+    constexpr int OP = BMB200_OP_AND_SUB;
+    extern __shared__ __align__(128) uint8_t dyn_smem[];
+    const uint32_t dyn_s = smem_u32(dyn_smem);
+    const uint32_t k_off = ((dyn_s + kLiveAlign - 1u) & ~(kLiveAlign - 1u)) - dyn_s;
+    if (k_off + kLiveAlign + (uint32_t)kPipeRingSmem > p.dyn_bytes) __trap();     // host and kernel disagree about the layout
+    uint32_t* K = reinterpret_cast<uint32_t*>(dyn_smem + k_off);
+    uint8_t* ring = dyn_smem + k_off + kLiveAlign;
+
+    __shared__ __align__(8) uint64_t s_full[kPipeStages], s_empty[kPipeStages], s_qfull[kPipeQueue], s_qempty[kPipeQueue];
+    __shared__ uint4 s_q[kPipeQueue];                       // (item | ~0 = end, bit stages, GAP bytes, first stage)
+    __shared__ uint32_t s_g1[kPipeMaxVec / 32];             // vector -> member of group1 (AND-SUB)
+    __shared__ uint32_t s_brole[2][kPipeMaxVec / 32];       // bit-block j of the column -> group1, one buffer per column parity
+    __shared__ uint32_t s_st[2][6];                         // flags, bit0, gap0, AND-group GAP blocks, non-FLAT, first GAP unit
+    __shared__ uint2 s_ag[2][kPipeMaxAndGap];               // AND-group GAP blocks of the column: (descriptor, end of its last 16-byte unit)
+    __shared__ uint32_t s_pc[kAggWarps], s_tr[kAggWarps], s_dg[kAggWarps];
+
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t M = p.set.n_vec;
+    const uint32_t n0 = p.goff[1], n1 = p.goff[2] - p.goff[1];
+    if (tid == 0) {
+        for (int s = 0; s < kPipeStages; ++s) { mbar_init(&s_full[s], 1u); mbar_init(&s_empty[s], kAggWarps); }
+        for (int q = 0; q < kPipeQueue; ++q) { mbar_init(&s_qfull[q], 1u); mbar_init(&s_qempty[q], kAggWarps); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    for (uint32_t i = tid; i < kPipeMaxVec / 32; i += kPipeThreads) { s_g1[i] = 0u; s_brole[0][i] = 0u; }
+    if (tid < 12) (&s_st[0][0])[tid] = (tid % 6 == 5) ? ~0u : 0u;
+    __syncthreads();
+    for (uint32_t k = n0 + tid; k < n0 + n1; k += kPipeThreads) { const uint32_t v = p.group[k]; atomicOr(&s_g1[v >> 5], 1u << (v & 31u)); }
+    __syncthreads();                                        // the last CTA-wide barrier: the producer warp leaves below
+
+    if (warp == kAggWarps) {                                // ---- producer (one lane) ----
+        if (lane != 0) return;
+        uint32_t seq = 0;
+        for (uint32_t qi = 0;; ++qi) {
+            const uint32_t qs = qi % kPipeQueue;
+            mbar_wait(&s_qempty[qs], ((qi / kPipeQueue) & 1u) ^ 1u);
+            const uint32_t item = atomicAdd(p.work_counter, 1u);
+            if (item >= p.n_cols) { s_q[qs] = make_uint4(~0u, 0u, 0u, 0u); mbar_arrive(&s_qfull[qs]); return; }
+            const uint32_t nb = p.nb_from + item;
+            const uint64_t b0 = p.set.bit_base[nb], g0 = p.set.gap_base[nb];
+            const uint32_t nbit = (uint32_t)(p.set.bit_base[nb + 1] - b0), gbytes = (uint32_t)((p.set.gap_base[nb + 1] - g0) * 16u);
+            s_q[qs] = make_uint4(item, nbit, gbytes, seq);
+            mbar_arrive(&s_qfull[qs]);
+            const uint8_t* bsrc = reinterpret_cast<const uint8_t*>(p.set.bit_pool + b0 * kBlockWords);
+            const uint8_t* gsrc = reinterpret_cast<const uint8_t*>(p.set.gap_pool + g0 * kGapUnit);
+            const uint32_t ns = nbit + (gbytes + kPipeStage - 1u) / kPipeStage;
+            for (uint32_t j = 0; j < ns; ++j, ++seq) {
+                const uint32_t s = seq % kPipeStages;
+                mbar_wait(&s_empty[s], ((seq / kPipeStages) & 1u) ^ 1u);
+                const uint32_t bytes = j < nbit ? kPipeStage : min(kPipeStage, gbytes - (j - nbit) * kPipeStage);
+                const uint8_t* src = j < nbit ? bsrc + (size_t)j * kPipeStage : gsrc + (size_t)(j - nbit) * kPipeStage;
+                mbar_arrive_expect_tx(&s_full[s], bytes);
+                bulk_g2s(ring + (size_t)s * kPipeStage, src, bytes, &s_full[s]);
+            }
+        }
+    }
+
+    // ---- consumers: tid < kAggThreads ----
+    uint4* K4 = reinterpret_cast<uint4*>(K);
+    uint32_t Ks, ring_s;
+    asm volatile("mov.u32 %0, %1;" : "=r"(Ks) : "r"(smem_u32(K)));
+    asm volatile("mov.u32 %0, %1;" : "=r"(ring_s) : "r"(smem_u32(ring)));
+    for (uint32_t qi = 0;; ++qi) {
+        const uint32_t b = qi & 1u, qs = qi % kPipeQueue;
+        K4[tid] = make_uint4(~0u, ~0u, ~0u, ~0u);           // live mask: every bit still a candidate
+        if (tid < 6) s_st[b ^ 1u][tid] = (tid == 5) ? ~0u : 0u;          // next column's counters (nobody reads them any more)
+        if (tid < (int)(kPipeMaxVec / 32)) s_brole[b ^ 1u][tid] = 0u;
+        mbar_wait(&s_qfull[qs], (qi / kPipeQueue) & 1u);
+        const uint4 e = s_q[qs];
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&s_qempty[qs]);
+        if (e.x == ~0u) break;
+        const uint32_t item = e.x, nbit = e.y, gbytes = e.z, seq0 = e.w;
+        const uint32_t nb = p.nb_from + item;
+        const uint32_t* drow = p.set.desc + (size_t)nb * M;
+        const uint16_t* gseg = p.set.gap_pool + p.set.gap_base[nb] * (size_t)kGapUnit;
+
+        // ---- classification by vector (every vector is a member: no member list to resolve) ----
+        uint32_t dv[kPipePerThr];
+        uint32_t fl = 0, nb0 = 0, ng0 = 0, nonflat = 0, lo = ~0u;
+#pragma unroll
+        for (int i = 0; i < kPipePerThr; ++i) {
+            const uint32_t v = (uint32_t)tid + (uint32_t)i * kAggThreads;
+            dv[i] = v < M ? drow[v] : BMB200_BLK_NULL;
+        }
+#pragma unroll
+        for (int i = 0; i < kPipePerThr; ++i) {
+            const uint32_t v = (uint32_t)tid + (uint32_t)i * kAggThreads;
+            if (v >= M) continue;
+            const uint32_t d = dv[i], kind = d & 3u;
+            const bool g1 = (s_g1[v >> 5] >> (v & 31u)) & 1u;
+            if (kind == BMB200_BLK_BIT) {
+                if (g1) atomicOr(&s_brole[b][((d >> 2) & (kPipeMaxVec - 1u)) >> 5], 1u << ((d >> 2) & 31u)); else ++nb0;
+            } else if (kind == BMB200_BLK_GAP) {
+                const uint32_t u = (d >> 2) & kRelMask;
+                if (g1) {
+                    if (!((d >> 2) & kEntFlat)) nonflat = 1u;         // the FLAT sweep reads SUB-group blocks in FLAT form only
+                } else {                                              // AND group: listed, applied from global memory and blanked in the stage
+                    ++ng0;
+                    const uint32_t k = atomicAdd(&s_st[b][3], 1u);
+                    if (k < kPipeMaxAndGap) s_ag[b][k] = make_uint2(d, (u * 16u + 2u * (d >> 31) + 2u * ((gseg[(size_t)u * kGapUnit + (d >> 31)] >> 3) + 1u) + 15u) & ~15u);
+                    else nonflat = 1u;
+                }
+                lo = min(lo, u);
+            } else if (kind == BMB200_BLK_NULL) {
+                if (!g1) fl |= kFlNull0;
+            } else {
+                fl |= g1 ? kFlFull1 : kFlFull0;
+            }
+        }
+        fl = __reduce_or_sync(0xffffffffu, fl); nonflat = __reduce_or_sync(0xffffffffu, nonflat); lo = __reduce_min_sync(0xffffffffu, lo);
+        nb0 = warp_sum(nb0); ng0 = warp_sum(ng0);
+        if (lane == 0) {
+            if (fl) atomicOr(&s_st[b][0], fl);
+            if (nb0) atomicAdd(&s_st[b][1], nb0);
+            if (ng0) atomicAdd(&s_st[b][2], ng0);
+            if (nonflat) s_st[b][4] = 1u;
+            if (lo != ~0u) atomicMin(&s_st[b][5], lo);
+        }
+        agg_sync<true>();
+        // FLAT: the whole GAP segment is a flat window of 1-run sources (headers, pads and tail fill decode to empty runs)
+        const bool flat = s_st[b][4] == 0u && s_st[b][5] == 0u;
+        const uint32_t nag = s_st[b][3];                         // <= kPipeMaxAndGap when flat
+
+        // ---- bit phase: stage j = bit-block j of the column ----
+        uint4 acc0 = make_uint4(~0u, ~0u, ~0u, ~0u);
+        uint4 acc1 = make_uint4(0u, 0u, 0u, 0u);
+        for (uint32_t j = 0; j < nbit; ++j) {
+            const uint32_t sq = seq0 + j, s = sq % kPipeStages;
+            mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
+            const uint4 v = lds128(ring_s + s * kPipeStage + (uint32_t)tid * 16u);
+            if ((s_brole[b][j >> 5] >> (j & 31u)) & 1u) acc_or(acc1, v); else acc_apply0<OP>(acc0, v);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&s_empty[s]);
+        }
+        {
+            uint4 l = K4[tid];
+            l.x &= acc0.x & ~acc1.x; l.y &= acc0.y & ~acc1.y; l.z &= acc0.z & ~acc1.z; l.w &= acc0.w & ~acc1.w;
+            K4[tid] = l;
+        }
+        agg_sync<true>();
+
+        // ---- GAP phase: GAP stage g belongs to warp g % 16 ----
+        const uint32_t ngs = (gbytes + kPipeStage - 1u) / kPipeStage;
+        if (flat) {
+            // a FLAT SUB-group block without lead pad starts with a 1-run whose pair slot holds the header: clear that whole run here
+#pragma unroll
+            for (int i = 0; i < kPipePerThr; ++i) {
+                const uint32_t d = dv[i], v = (uint32_t)tid + (uint32_t)i * kAggThreads;
+                if (v < M && (d & 3u) == BMB200_BLK_GAP && !(d >> 31) && ((s_g1[v >> 5] >> (v & 31u)) & 1u))
+                    apply_run<false>(Ks, 0u, gseg[(size_t)((d >> 2) & kRelMask) * kGapUnit + 1u]);
+            }
+            for (uint32_t i = (uint32_t)warp; i < nag; i += kAggWarps) {   // AND-group GAP blocks: their 0-runs, read in place
+                const uint32_t d = s_ag[b][i].x;
+                gap_scatter_gather<false>(Ks, gseg + (size_t)((d >> 2) & kRelMask) * kGapUnit + (d >> 31), 0u, lane);
+            }
+            uint32_t flat_mode = 0;
+            for (uint32_t g = (uint32_t)warp; g < ngs; g += kAggWarps) {
+                const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
+                mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
+                if (nag) {   // blank the staged bytes of AND-group blocks: as zero pairs the sweep reads no run in them
+                    const uint32_t st0 = g * kPipeStage, st1 = st0 + min(kPipeStage, gbytes - st0);
+                    for (uint32_t i = 0; i < nag; ++i) {
+                        const uint2 a = s_ag[b][i];
+                        const uint32_t bs = max(((a.x >> 2) & kRelMask) * 16u, st0), be = min(a.y, st1);
+                        for (uint32_t x = bs + 2u * (uint32_t)lane; x < be; x += 64u)
+                            asm volatile("st.shared.u16 [%0], %1;" :: "r"(ring_s + s * kPipeStage + (x - st0)), "h"((uint16_t)0) : "memory");
+                    }
+                    fence_proxy_async();     // generic writes before the stage is refilled by the async proxy
+                    __syncwarp();
+                }
+                if (flat_mode == 0u) {   // same one-way test-first switch as agg_kernel's FLAT consumer
+                    const uint32_t smp = lds32(Ks + ((((uint32_t)lane * 65u + g * 7u) & (kBlockWords - 1u)) << 2));
+                    flat_mode = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(smp)) < 256u ? 1u : 0u;
+                }
+                flat_sweep_fn(Ks, ring_s + s * kPipeStage + (uint32_t)lane * 16u, min(kPipeStage, gbytes - g * kPipeStage), (uint32_t)lane * 16u, flat_mode);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&s_empty[s], kAggWarps);
+            }
+        } else {
+            for (uint32_t g = (uint32_t)warp; g < ngs; g += kAggWarps) {      // release the staged segment unread
+                const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
+                mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
+                if (lane == 0) mbar_arrive(&s_empty[s], kAggWarps);
+            }
+#pragma unroll
+            for (int i = 0; i < kPipePerThr; ++i) {            // this warp's 32 vectors of trip i, one GAP block at a time
+                const uint32_t v = (uint32_t)tid + (uint32_t)i * kAggThreads;
+                uint32_t m = __ballot_sync(0xffffffffu, v < M && (dv[i] & 3u) == BMB200_BLK_GAP);
+                while (m) {
+                    const int l = __ffs(m) - 1; m &= m - 1u;
+                    const uint32_t d = __shfl_sync(0xffffffffu, dv[i], l);
+                    const uint32_t vl = v - (uint32_t)lane + (uint32_t)l;
+                    const uint32_t want = (s_g1[vl >> 5] >> (vl & 31u)) & 1u;   // AND group: 0-runs, SUB group: 1-runs
+                    gap_scatter_gather<false>(Ks, gseg + (size_t)((d >> 2) & kRelMask) * kGapUnit + (d >> 31), want, lane);
+                }
+            }
+        }
+        agg_sync<true>();
+
+        // ---- epilogue ----
+        const int state = and_state<OP>(s_st[b][0], s_st[b][1], s_st[b][2], n0, n1);
+        const uint4 R = state == 0 ? make_uint4(0u, 0u, 0u, 0u) : state == 1 ? make_uint4(~0u, ~0u, ~0u, ~0u) : K4[tid];
+        finish_block<true, true>(p, item, item, 0u, R, state, K, s_pc, s_tr, s_dg);
     }
 }
 

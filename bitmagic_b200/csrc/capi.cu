@@ -51,6 +51,8 @@ struct bmb200_ctx {
     int gap_mode = 0;                       // 0 = stream sorted GAP lists through the smem ring, 1 = always gather
     bool attr_set = false, merge_attr_set = false;
     size_t agg_dyn[4] = {};                 // dynamic shared memory per agg_kernel<OP> (set_agg_attrs)
+    size_t pipe_dyn = 0;                    // ... of agg_pipe_kernel
+    int agg_pipeline = 1;                   // 1 = whole-set AND-SUB takes agg_pipe_kernel, 0 = always agg_kernel
     int host_threads = 0;                   // host threads of bmb200_set_upload_vectors (0 = hardware concurrency, at most 64)
     uint8_t* h_ring[kStageSlots] = {};      // pinned staging ring of bmb200_set_upload_vectors (grow-only)
     size_t h_ring_cap = 0;
@@ -75,6 +77,7 @@ struct bmb200_set {
     SetView v{};
     bool owns = false;
     uint64_t n_bit_blocks = 0, n_gap_units = 0;
+    int flat_gaps = -1;                     // every GAP block in BMB200_DESC_GAP_FLAT form: 1 yes, 0 no, -1 not checked yet (flat_gap_set)
     uint64_t gap_pool_bytes = 0;            // readable bytes of gap_pool (with the allocation slack when owned)
     size_t cap_desc = 0, cap_base = 0, cap_bit = 0, cap_gap = 0;   // capacities when the arrays came from set_alloc (elements / blocks / units); 0 = not recyclable
 };
@@ -420,6 +423,7 @@ int bmb200_ctx_set_tuning(bmb200_ctx* ctx, int key, int value)
     if (key == BMB200_TUNE_GAP_MODE && (value == 0 || value == 1)) { ctx->gap_mode = value; return BMB200_OK; }
     if (key == BMB200_TUNE_CTAS_PER_SM && value >= 1 && value <= kCtasPerSm) { ctx->agg_ctas_per_sm = value; return BMB200_OK; }
     if (key == BMB200_TUNE_HOST_THREADS && value >= 0 && value <= 64) { ctx->host_threads = value; return BMB200_OK; }
+    if (key == BMB200_TUNE_AGG_PIPELINE && (value == 0 || value == 1)) { ctx->agg_pipeline = value; return BMB200_OK; }
     return BMB200_ERR_BADARG;
 }
 
@@ -1228,12 +1232,12 @@ static int result_alloc(bmb200_ctx* ctx, uint32_t n_cols, uint32_t n_groups, boo
 // dynamic shared memory per aggregation kernel: depends on its static size (the live mask is 8 KB aligned in the shared window)
 extern "C++" {
 template <typename KFn>
-static cudaError_t agg_attr_one(KFn fn, size_t reserved, size_t* dyn_out)
+static cudaError_t agg_attr_one(KFn fn, size_t reserved, size_t* dyn_out, size_t ring_bytes = kAggRingSmem)
 {
     cudaFuncAttributes fa;
     cudaError_t e = cudaFuncGetAttributes(&fa, fn);
     if (e != cudaSuccess) return e;
-    *dyn_out = agg_dyn_smem(fa.sharedSizeBytes, reserved);
+    *dyn_out = agg_dyn_smem(fa.sharedSizeBytes, reserved, ring_bytes);
     return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*dyn_out);
 }
 }
@@ -1246,7 +1250,42 @@ static void set_agg_attrs(bmb200_ctx* ctx, cudaError_t* e)
     if (*e == cudaSuccess) *e = agg_attr_one(agg_kernel<BMB200_OP_AND>, (size_t)reserved, &ctx->agg_dyn[BMB200_OP_AND]);
     if (*e == cudaSuccess) *e = agg_attr_one(agg_kernel<BMB200_OP_AND_SUB>, (size_t)reserved, &ctx->agg_dyn[BMB200_OP_AND_SUB]);
     if (*e == cudaSuccess) *e = agg_attr_one(agg_kernel<BMB200_OP_XOR>, (size_t)reserved, &ctx->agg_dyn[BMB200_OP_XOR]);
+    if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel, (size_t)reserved, &ctx->pipe_dyn, kPipeRingSmem);
     if (*e == cudaSuccess) ctx->attr_set = true;
+}
+
+// agg_pipe_kernel's inputs: one AND-SUB group whose group0 + group1 are every vector of the set exactly once, a set small enough
+// for its per-vector role table, and an AND group small enough that its GAP blocks of a column fit the kernel's list
+static bool whole_set(const bmb200_batch_args* a, uint32_t n_vec)
+{
+    if (a->n_groups != 1 || a->op != BMB200_OP_AND_SUB || n_vec == 0 || n_vec > kPipeMaxVec || a->offsets[0] != 0) return false;
+    if (a->offsets[1] > kPipeMaxAndGap) return false;
+    const uint32_t n = a->offsets[2];
+    if (n != n_vec) return false;
+    std::vector<bool> seen(n_vec, false);
+    for (uint32_t k = 0; k < n; ++k) {
+        if (seen[a->members[k]]) return false;
+        seen[a->members[k]] = true;
+    }
+    return true;
+}
+
+// Are all GAP blocks of the set in the FLAT form?  Checked once per set on the device (one pass over the descriptors, then a wait
+// for the answer) and remembered: a set's descriptors do not change after it is built.
+static bool flat_gap_set(bmb200_ctx* ctx, const bmb200_set* set)
+{
+    bmb200_set* s = const_cast<bmb200_set*>(set);
+    if (s->flat_gaps < 0) {
+        uint32_t bad = 1u;
+        const size_t n = (size_t)set->v.n_vec * set->v.n_blocks;
+        const uint32_t grid = (uint32_t)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 8);
+        if (cudaMemsetAsync(ctx->d_work + 1, 0, 4, ctx->stream) != cudaSuccess) return false;
+        if (grid) desc_flat_check_kernel<<<grid, 256, 0, ctx->stream>>>(set->v.desc, n, ctx->d_work + 1);
+        if (cudaMemcpyAsync(&bad, ctx->d_work + 1, 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess ||
+            cudaStreamSynchronize(ctx->stream) != cudaSuccess) { cudaGetLastError(); return false; }
+        s->flat_gaps = bad ? 0 : 1;
+    }
+    return s->flat_gaps == 1;
 }
 
 int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_batch_args* a, bmb200_result** inout)
@@ -1332,16 +1371,23 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     p.gap_mode = (uint32_t)ctx->gap_mode; p.gap_pool_bytes = set->gap_pool_bytes;
     cudaError_t ae = cudaSuccess; set_agg_attrs(ctx, &ae);
     if (ae != cudaSuccess) { ctx->last_err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(ae); if (!*inout) bmb200_result_free(r); return BMB200_ERR_CUDA; }
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
+    uint32_t sms = (uint32_t)ctx->sm_count;
     if (ctx->comm.comm && ctx->comm.nranks > 1 && ctx->sm_count > 8) {
         // sharded runs: the all-gather of the previous step has to find SMs while this (persistent, SM-filling) kernel runs, or it
         // waits for the gap between two aggregation kernels and stretches it; BMB200_AGG_RESERVE_SMS leaves that many SMs free
         static const int reserve = []() { const char* e = getenv("BMB200_AGG_RESERVE_SMS"); return e ? atoi(e) : 0; }();
-        if (reserve > 0 && reserve < ctx->sm_count) grid = (uint32_t)((ctx->sm_count - reserve) * ctx->agg_ctas_per_sm);
+        if (reserve > 0 && reserve < ctx->sm_count) sms = (uint32_t)(ctx->sm_count - reserve);
     }
+    uint32_t grid = sms * (uint32_t)ctx->agg_ctas_per_sm;
     if (grid > n_cols) grid = n_cols;
     if (a->op != BMB200_OP_SHIFT_R_AND) p.dyn_bytes = (uint32_t)ctx->agg_dyn[a->op];
-    switch (a->op) {
+    if (ctx->agg_pipeline && ctx->gap_mode == 0 && set->n_gap_units && whole_set(a, set->v.n_vec) && flat_gap_set(ctx, set)) {
+        // one AND-SUB group naming every vector once: a producer warp streams whole columns (agg_pipe_kernel), one CTA per SM.
+        // OR stays on agg_kernel: its whole-set workloads measured at par or slower through the ring (DESIGN §3.1a)
+        p.dyn_bytes = (uint32_t)ctx->pipe_dyn;
+        const uint32_t pgrid = sms < n_cols ? sms : n_cols;
+        agg_pipe_kernel<<<pgrid, kPipeThreads, ctx->pipe_dyn, ctx->stream>>>(p);
+    } else switch (a->op) {
     case BMB200_OP_OR:      agg_kernel<BMB200_OP_OR><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_OR], ctx->stream>>>(p); break;
     case BMB200_OP_AND:     agg_kernel<BMB200_OP_AND><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_AND], ctx->stream>>>(p); break;
     case BMB200_OP_AND_SUB: agg_kernel<BMB200_OP_AND_SUB><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_AND_SUB], ctx->stream>>>(p); break;

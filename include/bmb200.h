@@ -110,6 +110,8 @@ typedef struct bmb200_rs     bmb200_rs;      /* device-resident rank-select inde
  *           every kernel accepts every form; the library's own packers and bmb200_synth_set write FLAT.
  *   bit segment of column nb = bit_pool blocks [bit_base[nb], bit_base[nb+1])
  *   GAP segment of column nb = gap_pool units  [gap_base[nb], gap_base[nb+1])
+ *   Every block of a segment belongs to exactly one vector of its column (no unreferenced or shared blocks): an aggregation
+ *   over the whole set reads the segments as they lie.
  * All blocks of one column are contiguous, so one CTA streams one column.
  */
 typedef struct bmb200_packed_set {
@@ -180,6 +182,7 @@ int bmb200_device_info(const bmb200_ctx* ctx, int* sm_count, int* cc_major, int*
 #define BMB200_TUNE_GAP_MODE     0
 #define BMB200_TUNE_CTAS_PER_SM  1
 #define BMB200_TUNE_HOST_THREADS 2   /* host threads that pack blocks in bmb200_set_upload_vectors: 0 = all cores (at most 64) */
+#define BMB200_TUNE_AGG_PIPELINE 3   /* 1 (default) = whole-set AND-SUB aggregations take the streamed-column kernel, 0 = never (A/B reference) */
 int bmb200_ctx_set_tuning(bmb200_ctx* ctx, int key, int value);
 /* pin the CALLING thread (and the threads it starts later, e.g. the packers of bmb200_set_upload_vectors) to the CPUs of the NUMA
  * node this context's GPU hangs off, so that pinned staging memory is allocated next to the GPU's PCIe root.  *node = the node, or
