@@ -12,7 +12,7 @@ from pathlib import Path
 import numpy as np
 
 _HERE = Path(__file__).resolve().parent
-LIB_PATH = Path(os.environ.get("BMB200_LIB", str(_HERE / "libbmb200.so")))   # override only for kernel-variant experiments
+LIB_PATH = Path(os.environ.get("BMB200_LIB", str(_HERE / "libbmb200.so")))   # load another build, e.g. to compare two builds on the same inputs
 
 # ---- constants (mirror include/bmb200.h) ----
 OK = 0

@@ -43,43 +43,17 @@ namespace bmb200 {
 constexpr int kAggThreads = 512;
 constexpr int kAggWarps   = kAggThreads / 32;
 constexpr int kAggChunk   = 1024;   // group members classified per pass (AND-SUB)
-#ifndef BMB200_AGG_CHUNK_WIDE
-#define BMB200_AGG_CHUNK_WIDE 1408
-#endif
-constexpr int kAggChunkWide = BMB200_AGG_CHUNK_WIDE;  // ... in the one-group kernels (OR / AND / XOR)
+constexpr int kAggChunkWide = 1408; // ... in the one-group kernels (OR / AND / XOR)
 
-// build-time variants (scripts/build_variants.sh explores them; defaults = best measured)
-#ifndef BMB200_CTAS_PER_SM       /* resident CTAs per SM the kernel is shaped for: 2 (64 regs, 4-stage ring) or 3 (40 regs, 3-stage ring) */
-#define BMB200_CTAS_PER_SM 2
-#endif
-#ifndef BMB200_GAP_STAGES
-#define BMB200_GAP_STAGES (BMB200_CTAS_PER_SM >= 3 ? 3 : 4)
-#endif
-#ifndef BMB200_BIT_UNROLL        /* bit-blocks in flight per thread */
-#define BMB200_BIT_UNROLL 4
-#endif
-#ifndef BMB200_GAP_CHUNK
-#define BMB200_GAP_CHUNK 16384
-#endif
-#ifndef BMB200_LANES_PER_BLOCK   /* lanes that share one GAP block in the streamed scatter: 32, 16, 8 or 4 */
-#define BMB200_LANES_PER_BLOCK 16
-#endif
-#ifndef BMB200_VAR_UNROLL2       /* two scatter steps per loop trip: both loads issued before the first red */
-#define BMB200_VAR_UNROLL2 1
-#endif
-#ifndef BMB200_VAR_SLEEP_NS
-#define BMB200_VAR_SLEEP_NS 64
-#endif
-constexpr uint32_t kLanesPerBlock = BMB200_LANES_PER_BLOCK;      // `lane` below = lane inside its group
-constexpr uint32_t kGroupsPerWarp = 32u / kLanesPerBlock;
-constexpr int      kGapStages     = BMB200_GAP_STAGES;
-constexpr uint32_t kGapChunkBytes = BMB200_GAP_CHUNK;
-constexpr uint32_t kRingBytes     = kGapStages * kGapChunkBytes;   // 64 KB (48 KB with 3 stages); offsets wrap by modulo
-constexpr int      kCtasPerSm     = BMB200_CTAS_PER_SM;
-constexpr int      kBitUnroll     = BMB200_BIT_UNROLL;
-constexpr uint32_t kRingWords     = kRingBytes / 4;
+constexpr int      kCtasPerSm     = 2;                             // resident CTAs per SM agg_kernel is shaped for (64 registers)
+constexpr int      kBitUnroll     = 4;                             // bit-blocks in flight per thread
+constexpr uint32_t kLanesPerBlock = 16;                            // lanes that share one GAP block in the streamed scatter
+constexpr uint32_t kGroupsPerWarp = 32u / kLanesPerBlock;          // `lane` below = lane inside its group
+constexpr uint32_t kVarSleepNs    = 64;                            // back-off of an mbarrier wait
+constexpr int      kGapStages     = 4;
+constexpr uint32_t kGapChunkBytes = 16384;
+constexpr uint32_t kRingBytes     = kGapStages * kGapChunkBytes;   // 64 KB; offsets wrap by modulo
 constexpr uint32_t kGapMaxBytes   = 2560;                          // gap_max_buff_len * 2
-constexpr int      kMaxChunks     = (kAggChunk * 4096) / (int)kGapChunkBytes + 4;      // streamed only when span <= n * 4096
 constexpr uint32_t kRingTail      = kGapMaxBytes + 512;           // tail mirror (+ over-read slack of one 64-run step)
 constexpr size_t   kAggRingSmem   = kRingBytes + kRingTail;       // blocks never wrap
 // dynamic shared memory of agg_kernel: [pad to the next 8 KB boundary of the shared WINDOW][live mask L, 8 KB][ring + tail].
@@ -96,19 +70,14 @@ __host__ inline size_t agg_dyn_smem(size_t static_bytes, size_t reserved_bytes, 
 }
 // FLAT consumer: the ring is cut into one private slot per warp; warp w streams chunks w, w+16, ... of the window through
 // its own slot and its own mbarrier -- no cross-warp hand-off, the per-chunk overhead is paid once per slot, not 16 times
-#ifndef BMB200_FLAT_SLOTS         /* private slots per warp: 2 = one being consumed while the other one fills, 1 = one 4 KB slot, 0 = by window size */
-#define BMB200_FLAT_SLOTS 0
-#endif
 constexpr uint32_t kFlatSlots     = 2u;                                      // barriers per warp (the most slots a warp's region is cut into)
 constexpr uint32_t kFlatWarpBytes = kRingBytes / kAggWarps;                  // 4 KB of the 64 KB ring per warp
 static_assert(kFlatWarpBytes % 2048u == 0, "a warp's ring region is cut into 1 or 2 slots of whole KB");
 // The region is used as TWO 2 KB slots (one fills while the other is consumed) or as ONE 4 KB slot, chosen per window: the per-slot
 // control code (claim, mbarrier wait, refill) is ~18 % of the GAP-phase instructions with 2 KB slots, so long windows (config 5: 2.7 MB
 // per column) take 4 KB pieces; short ones (config 3: ~0.4 MB per column = 6 pieces per warp) keep 2 KB pieces, whose finer claim
-// granularity balances the 16 warps better.  BMB200_FLAT_SLOTS = 1 / 2 forces one form, 0 = choose by window size.
-#ifndef BMB200_FLAT_BIG_WINDOW
-#define BMB200_FLAT_BIG_WINDOW (640u << 10)   /* >= 10 pieces of 4 KB for each of the 16 warps */
-#endif
+// granularity balances the 16 warps better.
+constexpr uint32_t kFlatBigWindow = 640u << 10;                              // >= 10 pieces of 4 KB for each of the 16 warps
 
 struct AggParams {
     SetView   set;
@@ -147,11 +116,13 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count)
 {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory");
 }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes)
+// The raw forms take 32-bit shared-window addresses (callers that keep them in registers); the others convert a generic pointer.
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes)
 {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(bytes) : "memory");
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) { mbar_arrive_expect_tx(smem_u32(bar), bytes); }
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
 {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
@@ -160,28 +131,22 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
         "@p bra WAIT_DONE;\n\t"
         "nanosleep.u32 %2;\n\t"
         "bra WAIT_LOOP;\n\t"
-        "WAIT_DONE:\n\t}\n" :: "r"(smem_u32(bar)), "r"(parity), "n"(BMB200_VAR_SLEEP_NS) : "memory");
+        "WAIT_DONE:\n\t}\n" :: "r"(bar), "r"(parity), "n"(kVarSleepNs) : "memory");
 }
-__device__ __forceinline__ void mbar_wait_a(uint32_t bar_addr, uint32_t parity)       // same, raw shared-window address
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_LOOP_A:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra WAIT_DONE_A;\n\t"
-        "nanosleep.u32 %2;\n\t"
-        "bra WAIT_LOOP_A;\n\t"
-        "WAIT_DONE_A:\n\t}\n" :: "r"(bar_addr), "r"(parity), "n"(BMB200_VAR_SLEEP_NS) : "memory");
-}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) { mbar_wait(smem_u32(bar), parity); }
 __device__ __forceinline__ uint32_t atoms_add(uint32_t a, uint32_t v)
 {
     uint32_t old; asm volatile("atom.shared.add.u32 %0, [%1], %2;" : "=r"(old) : "r"(a), "r"(v) : "memory"); return old;
 }
 __device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" :: "r"(a), "r"(v) : "memory"); }
-__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
+__device__ __forceinline__ void bulk_g2s(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar)
 {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+                 :: "r"(smem_dst), "l"(gsrc), "r"(bytes), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar)
+{
+    bulk_g2s(smem_u32(smem_dst), gsrc, bytes, smem_u32(bar));
 }
 __device__ __forceinline__ void fence_proxy_async()
 {
@@ -294,9 +259,7 @@ __device__ __noinline__ void flat_quad_tail(uint32_t Ls, const uint4 q)   // rar
 {
     flat_pair_tail(Ls, q.x); flat_pair_tail(Ls, q.y); flat_pair_tail(Ls, q.z); flat_pair_tail(Ls, q.w);
 }
-#ifndef BMB200_FLAT_LEAN          /* 1: lean pair decode -- hi - lo by one dp2a, word address by one and-or (L is 8 KB aligned) */
-#define BMB200_FLAT_LEAN 1
-#endif
+// Pair decode: hi - lo by one dp2a, word address by one and-or (L is 8 KB aligned).
 // hi16(w) - lo16(w) in one instruction: dp2a.lo = c + lo16(a) * sbyte0(b) + hi16(a) * sbyte1(b) with b = (+1, -1)   (SASS IDP.2A)
 __device__ __forceinline__ int pair_width(uint32_t w)
 {
@@ -318,21 +281,12 @@ __device__ __forceinline__ void flat_quad(uint32_t Ls, const uint4& q)
     uint32_t a[4], m[4], nm[4], reach = 0;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-#if BMB200_FLAT_LEAN
         const uint32_t t = w[i] + 1u;                                         // low half = run start s = lo + 1 (s == 65536 wraps to 0: pad / terminator, mask 0)
         const uint32_t sb = t & 31u;
         const uint32_t wd = (uint32_t)max(pair_width(w[i]), 0);               // wd == 0: no run
         m[i] = bmsk(sb, wd);
         nm[i] = ~m[i];
         a[i] = and_or(t >> 3, 0x1ffcu, Ls);
-#else
-        const uint32_t lo = w[i] & 0xffffu, hi = w[i] >> 16;
-        const uint32_t s = lo + 1u, sb = s & 31u;
-        const uint32_t wd = (uint32_t)max((int)hi - (int)lo, 0);              // wd == 0: no run
-        m[i] = bmsk(sb, wd);
-        nm[i] = ~m[i];
-        a[i] = Ls + ((s >> 3) & 0x1ffcu);                                     // s == 65536 (pad / terminator) wraps to word 0, mask 0
-#endif
         reach = max(reach, sb + wd);
     }
     if (TEST) {
@@ -364,17 +318,19 @@ __device__ __forceinline__ void flat_sweep_mode(uint32_t Ls, uint32_t src, uint3
     if (h + lane_off < bytes)        { const uint4 qa = lds128(src + h);        flat_quad<MODE>(Ls, qa); }     // last, partial KB of the window
     if (h + 512u + lane_off < bytes) { const uint4 qb = lds128(src + h + 512u); flat_quad<MODE>(Ls, qb); }
 }
-#ifndef BMB200_FLAT_OOL           /* 1: one out-of-line copy of the sweep per kernel; 0: inlined at every call site */
-#define BMB200_FLAT_OOL 1
-#endif
-#if BMB200_FLAT_OOL
-__device__ __noinline__
-#else
-__device__ __forceinline__
-#endif
-void flat_sweep_fn(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off, uint32_t mode)
+__device__ __noinline__ void flat_sweep_fn(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off, uint32_t mode)
 {
     if (mode) flat_sweep_mode<1>(Ls, src, bytes, lane_off); else flat_sweep_mode<0>(Ls, src, bytes, lane_off);
+}
+// The sweep's form for one column, re-sampled before each piece until it switches (warp-uniform): a 1024-bit sample of L (piece
+// number c varies the sample); below 25 % alive the test-first form wins (one shared load, rarely an atomic).  Bits of L only ever
+// get cleared, so the switch is one-way per column.
+__device__ __forceinline__ void flat_update_mode(uint32_t& mode, uint32_t Ls, uint32_t lane, uint32_t c)
+{
+    if (mode == 0u) {
+        const uint32_t smp = lds32(Ls + (((lane * 65u + c * 7u) & (kBlockWords - 1u)) << 2));
+        mode = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(smp)) < 256u ? 1u : 0u;
+    }
 }
 
 // GAP format (src/bmfunc.h:1696-1725): buf[0] = header (bit0 first-run value, len = hdr>>3),
@@ -399,8 +355,8 @@ __device__ __forceinline__ void gap_scatter_ring(uint32_t Ks, uint32_t ba, uint3
     const bool odd = ((hdr & 1u) == want);
     const uint32_t nsel = odd ? (len + 1u) >> 1 : len >> 1;
     const uint32_t A0 = h + (odd ? 0u : 2u);
+    // two scatter steps per loop trip: both loads are issued before the first red
     if ((A0 & 2u) == 0u) {
-#if BMB200_VAR_UNROLL2
         for (uint32_t j = lane; j < nsel; j += 2u * kLanesPerBlock) {
             const uint32_t a = A0 + 4u * j;
             const bool v1 = (j + kLanesPerBlock < nsel);
@@ -409,14 +365,7 @@ __device__ __forceinline__ void gap_scatter_ring(uint32_t Ks, uint32_t ba, uint3
             apply_run<XOR>(Ks, (odd && j == 0u) ? 0u : (w0 & 0xffffu) + 1u, w0 >> 16);
             if (v1) apply_run<XOR>(Ks, (w1 & 0xffffu) + 1u, w1 >> 16);
         }
-#else
-        for (uint32_t j = lane; j < nsel; j += kLanesPerBlock) {
-            const uint32_t w = lds32(A0 + 4u * j);
-            apply_run<XOR>(Ks, (odd && j == 0u) ? 0u : (w & 0xffffu) + 1u, w >> 16);
-        }
-#endif
     } else {
-#if BMB200_VAR_UNROLL2
         for (uint32_t j = lane; j < nsel; j += 2u * kLanesPerBlock) {
             const uint32_t a = A0 + 4u * j;
             const bool v1 = (j + kLanesPerBlock < nsel);
@@ -425,13 +374,6 @@ __device__ __forceinline__ void gap_scatter_ring(uint32_t Ks, uint32_t ba, uint3
             apply_run<XOR>(Ks, (odd && j == 0u) ? 0u : s0 + 1u, e0);
             if (v1) apply_run<XOR>(Ks, s1 + 1u, e1);
         }
-#else
-        for (uint32_t j = lane; j < nsel; j += kLanesPerBlock) {
-            const uint32_t a = A0 + 4u * j;
-            const uint32_t sv = lds16(a), ev = lds16(a + 2u);
-            apply_run<XOR>(Ks, (odd && j == 0u) ? 0u : sv + 1u, ev);
-        }
-#endif
     }
 }
 
@@ -818,7 +760,7 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
             // FLAT: warps claim pieces of the window from a shared counter (one claim = kFlatSlots consecutive chunks, one per
             // private slot) and pull them through their slots
             auto flat_big = [&](uint32_t wbytes) -> bool {       // uniform: one 4 KB slot per warp instead of two 2 KB slots
-                return BMB200_FLAT_SLOTS == 1 ? true : BMB200_FLAT_SLOTS == 2 ? false : wbytes >= (uint32_t)BMB200_FLAT_BIG_WINDOW;
+                return wbytes >= kFlatBigWindow;
             };
             auto flat_claim = [&](auto S) -> uint32_t {          // whole warp; returns the first chunk of the claimed piece (S chunks)
                 uint32_t c = 0;
@@ -832,10 +774,9 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
                     const uint32_t bytes = min(kChunk, wbytes - off);
                     const uint32_t bar = wfull_s + 8u * k;
                     fence_proxy_async();
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(bar), "r"(bytes) : "memory");
-                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 :: "r"(ring_s + (uint32_t)warp * kFlatWarpBytes + k * kChunk),
-                                    "l"(reinterpret_cast<const uint8_t*>(gseg) + (size_t)wlo * 16u + off), "r"(bytes), "r"(bar) : "memory");
+                    mbar_arrive_expect_tx(bar, bytes);
+                    bulk_g2s(ring_s + (uint32_t)warp * kFlatWarpBytes + k * kChunk,
+                             reinterpret_cast<const uint8_t*>(gseg) + (size_t)wlo * 16u + off, bytes, bar);
                 }
             };
             auto flat_setup = [&](auto S, uint32_t wlo, uint32_t wbytes) {
@@ -915,13 +856,9 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
                     for (uint32_t k = 0; k < kS; ++k) {
                         const uint32_t c = wchunk[k];
                         if (c < nfc) {
-                            mbar_wait_a(wfull_s + 8u * k, (wphase >> k) & 1u); wphase ^= 1u << k;
+                            mbar_wait(wfull_s + 8u * k, (wphase >> k) & 1u); wphase ^= 1u << k;
                             const uint32_t bytes = min(kChunk, wbytes - c * kChunk);
-                            if (flat_mode == 0u) {   // 1024-bit sample of L: below 25 % alive the test-first form wins (one shared load, rarely
-                                                // an atomic); bits of L only ever get cleared, so the switch is one-way per column
-                                const uint32_t smp = lds32(Ks + ((((uint32_t)lane * 65u + c * 7u) & (kBlockWords - 1u)) << 2));
-                                flat_mode = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(smp)) < 256u ? 1u : 0u;
-                            }
+                            flat_update_mode(flat_mode, Ks, (uint32_t)lane, c);
                             flat_sweep_fn(Ks, ring_s + (uint32_t)warp * kFlatWarpBytes + k * kChunk + (uint32_t)lane * 16u, bytes, (uint32_t)lane * 16u, flat_mode);
                             __syncwarp();
                         }
@@ -1233,10 +1170,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
                     fence_proxy_async();     // generic writes before the stage is refilled by the async proxy
                     __syncwarp();
                 }
-                if (flat_mode == 0u) {   // same one-way test-first switch as agg_kernel's FLAT consumer
-                    const uint32_t smp = lds32(Ks + ((((uint32_t)lane * 65u + g * 7u) & (kBlockWords - 1u)) << 2));
-                    flat_mode = __reduce_add_sync(0xffffffffu, (uint32_t)__popc(smp)) < 256u ? 1u : 0u;
-                }
+                flat_update_mode(flat_mode, Ks, (uint32_t)lane, g);
                 flat_sweep_fn(Ks, ring_s + s * kPipeStage + (uint32_t)lane * 16u, min(kPipeStage, gbytes - g * kPipeStage), (uint32_t)lane * 16u, flat_mode);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&s_empty[s], kAggWarps);

@@ -1241,17 +1241,71 @@ static cudaError_t agg_attr_one(KFn fn, size_t reserved, size_t* dyn_out, size_t
     return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*dyn_out);
 }
 }
+// agg_kernel<op> by op (BMB200_OP_OR .. BMB200_OP_XOR); ctx->agg_dyn is indexed the same way
+static void (*const kAggKernels[4])(const AggParams) = {
+    agg_kernel<BMB200_OP_OR>, agg_kernel<BMB200_OP_AND>, agg_kernel<BMB200_OP_AND_SUB>, agg_kernel<BMB200_OP_XOR>};
+
 static void set_agg_attrs(bmb200_ctx* ctx, cudaError_t* e)
 {
     if (ctx->attr_set) return;
     int reserved = 1024;
     if (cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, ctx->device) != cudaSuccess) { cudaGetLastError(); reserved = 1024; }
-    *e = agg_attr_one(agg_kernel<BMB200_OP_OR>, (size_t)reserved, &ctx->agg_dyn[BMB200_OP_OR]);
-    if (*e == cudaSuccess) *e = agg_attr_one(agg_kernel<BMB200_OP_AND>, (size_t)reserved, &ctx->agg_dyn[BMB200_OP_AND]);
-    if (*e == cudaSuccess) *e = agg_attr_one(agg_kernel<BMB200_OP_AND_SUB>, (size_t)reserved, &ctx->agg_dyn[BMB200_OP_AND_SUB]);
-    if (*e == cudaSuccess) *e = agg_attr_one(agg_kernel<BMB200_OP_XOR>, (size_t)reserved, &ctx->agg_dyn[BMB200_OP_XOR]);
+    *e = cudaSuccess;
+    for (int op = 0; op < 4 && *e == cudaSuccess; ++op) *e = agg_attr_one(kAggKernels[op], (size_t)reserved, &ctx->agg_dyn[op]);
     if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel, (size_t)reserved, &ctx->pipe_dyn, kPipeRingSmem);
     if (*e == cudaSuccess) ctx->attr_set = true;
+}
+
+// agg_kernel<op> on `grid` CTAs with the dynamic shared memory set_agg_attrs sized for it
+static void launch_agg_kernel(bmb200_ctx* ctx, int op, uint32_t grid, AggParams& p)
+{
+    p.dyn_bytes = (uint32_t)ctx->agg_dyn[op];
+    kAggKernels[op]<<<grid, kAggThreads, ctx->agg_dyn[op], ctx->stream>>>(p);
+}
+
+// The AggParams of a launch that writes result r from set `set`; the caller adds its groups and whatever else differs
+static AggParams agg_params(const bmb200_ctx* ctx, const bmb200_set* set, const bmb200_result* r, uint32_t nb_from, uint32_t cols,
+                            bool compress, bool store)
+{
+    AggParams p{};
+    p.set = set->v; p.nb_from = nb_from; p.n_cols = cols;
+    p.compress = compress ? 1u : 0u; p.store_blocks = store ? 1u : 0u;
+    p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
+    p.total = r->total; p.work_counter = ctx->d_work;
+    p.gap_mode = (uint32_t)ctx->gap_mode; p.gap_pool_bytes = set->gap_pool_bytes;
+    return p;
+}
+
+// Stages the words a[0..na) b[0..nb) into ctx->d_group through the pinned buffer h_group (grown to at least max(1024, n) words) and
+// queues their upload.  With `reuse` the words are an aggregate member list: when they equal the list already resident (last_group)
+// nothing is uploaded and the stream is not synchronised, otherwise they are recorded as the resident list.  Without it the buffer
+// no longer holds member ids.
+static int stage_group(bmb200_ctx* ctx, const uint32_t* a, size_t na, const uint32_t* b, size_t nb, bool reuse)
+{
+    const size_t n = na + nb;
+    if (n > ctx->group_cap) {
+        cudaStreamSynchronize(ctx->stream);
+        cudaFree(ctx->d_group); if (ctx->h_group) cudaFreeHost(ctx->h_group);
+        ctx->d_group = nullptr; ctx->h_group = nullptr; ctx->group_cap = 0; ctx->last_group.clear();
+        const size_t cap = n < 1024 ? 1024 : n;
+        if (cudaMalloc((void**)&ctx->d_group, cap * 4) != cudaSuccess || cudaMallocHost((void**)&ctx->h_group, cap * 4) != cudaSuccess) {
+            ctx->last_err = "group buffer allocation"; return BMB200_ERR_BADALLOC;
+        }
+        ctx->group_cap = cap;
+    }
+    if (reuse && ctx->last_group.size() == n &&
+        (!na || memcmp(ctx->last_group.data(), a, na * 4) == 0) && (!nb || memcmp(ctx->last_group.data() + na, b, nb * 4) == 0))
+        return BMB200_OK;
+    ctx->last_group.clear();
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);     // the staging buffer may still feed a previous launch
+    if (e == cudaSuccess) {
+        if (na) memcpy(ctx->h_group, a, na * 4);
+        if (nb) memcpy(ctx->h_group + na, b, nb * 4);
+        e = cudaMemcpyAsync(ctx->d_group, ctx->h_group, n * 4, cudaMemcpyHostToDevice, ctx->stream);
+    }
+    if (e != cudaSuccess) { ctx->last_err = std::string("group upload: ") + cudaGetErrorString(e); return BMB200_ERR_CUDA; }
+    if (reuse) { try { ctx->last_group.assign(ctx->h_group, ctx->h_group + n); } catch (...) { ctx->last_group.clear(); } }
+    return BMB200_OK;
 }
 
 // agg_pipe_kernel's inputs: one AND-SUB group whose group0 + group1 are every vector of the set exactly once, a set small enough
@@ -1318,6 +1372,7 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
         int rc = result_alloc(ctx, n_cols, ng, store, store && compress, or_target, &r);
         if (rc) return rc;
     }
+    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
     r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
     if (r->total_inline && ctx->comm.comm) {
         r->xflip = (r->xflip + 1u) % (uint32_t)CommState::kSlots;
@@ -1328,49 +1383,18 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     }
 
     // member ids + offsets -> device (pinned staging keeps the copy asynchronous; skipped when unchanged)
-    const size_t nwords = nmem + 2 * (size_t)ng + 1;
-    if (nwords > ctx->group_cap) {
-        cudaStreamSynchronize(ctx->stream);
-        cudaFree(ctx->d_group); if (ctx->h_group) cudaFreeHost(ctx->h_group);
-        ctx->d_group = nullptr; ctx->h_group = nullptr; ctx->group_cap = 0; ctx->last_group.clear();
-        size_t cap = nwords < 1024 ? 1024 : nwords;
-        if (cudaMalloc((void**)&ctx->d_group, cap * 4) != cudaSuccess || cudaMallocHost((void**)&ctx->h_group, cap * 4) != cudaSuccess) {
-            ctx->last_err = "group buffer allocation"; if (!*inout) bmb200_result_free(r); return BMB200_ERR_BADALLOC;
-        }
-        ctx->group_cap = cap;
-    }
-    const bool same = ctx->last_group.size() == nwords &&
-                      (!nmem || memcmp(ctx->last_group.data(), a->members, nmem * 4) == 0) &&
-                      memcmp(ctx->last_group.data() + nmem, a->offsets, (2 * (size_t)ng + 1) * 4) == 0;
-    if (!same) {
-        cudaStreamSynchronize(ctx->stream);    // the staging buffer may still feed a previous launch
-        if (nmem) memcpy(ctx->h_group, a->members, nmem * 4);
-        memcpy(ctx->h_group + nmem, a->offsets, (2 * (size_t)ng + 1) * 4);
-        ctx->last_group.clear();
-    }
-    {   // a freshly allocated result must not leak when one of these fails
-        cudaError_t ce = cudaSuccess;
-        if (!same) ce = cudaMemcpyAsync(ctx->d_group, ctx->h_group, nwords * 4, cudaMemcpyHostToDevice, ctx->stream);
-        if (ce == cudaSuccess) ce = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
-        if (ce == cudaSuccess) ce = cudaMemsetAsync(r->total, 0, 8 * (size_t)ng, ctx->stream);
-        if (ce == cudaSuccess && or_target) ce = cudaMemsetAsync(r->or_blocks, 0, (size_t)cols * BMB200_BLOCK_BYTES, ctx->stream);
-        if (ce != cudaSuccess) {
-            ctx->last_err = std::string("aggregate: ") + cudaGetErrorString(ce);
-            if (!*inout) bmb200_result_free(r);
-            return BMB200_ERR_CUDA;
-        }
-        if (!same) { try { ctx->last_group.assign(ctx->h_group, ctx->h_group + nwords); } catch (...) { ctx->last_group.clear(); } }
-    }
+    int rc = stage_group(ctx, a->members, nmem, a->offsets, 2 * (size_t)ng + 1, true);
+    if (rc) return bail(rc);
+    cudaError_t ce = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
+    if (ce == cudaSuccess) ce = cudaMemsetAsync(r->total, 0, 8 * (size_t)ng, ctx->stream);
+    if (ce == cudaSuccess && or_target) ce = cudaMemsetAsync(r->or_blocks, 0, (size_t)cols * BMB200_BLOCK_BYTES, ctx->stream);
+    if (ce != cudaSuccess) { ctx->last_err = std::string("aggregate: ") + cudaGetErrorString(ce); return bail(BMB200_ERR_CUDA); }
 
-    AggParams p{};
-    p.set = set->v; p.group = ctx->d_group; p.goff = ctx->d_group + nmem; p.n_groups = ng;
-    p.nb_from = a->nb_from; p.n_cols = cols;
-    p.compress = compress ? 1u : 0u; p.store_blocks = store ? 1u : 0u;
-    p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
-    p.total = r->total; p.work_counter = ctx->d_work; p.or_blocks = or_target ? r->or_blocks : nullptr;
-    p.gap_mode = (uint32_t)ctx->gap_mode; p.gap_pool_bytes = set->gap_pool_bytes;
-    cudaError_t ae = cudaSuccess; set_agg_attrs(ctx, &ae);
-    if (ae != cudaSuccess) { ctx->last_err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(ae); if (!*inout) bmb200_result_free(r); return BMB200_ERR_CUDA; }
+    AggParams p = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
+    p.group = ctx->d_group; p.goff = ctx->d_group + nmem; p.n_groups = ng;
+    p.or_blocks = or_target ? r->or_blocks : nullptr;
+    set_agg_attrs(ctx, &ce);
+    if (ce != cudaSuccess) { ctx->last_err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(ce); return bail(BMB200_ERR_CUDA); }
     uint32_t sms = (uint32_t)ctx->sm_count;
     if (ctx->comm.comm && ctx->comm.nranks > 1 && ctx->sm_count > 8) {
         // sharded runs: the all-gather of the previous step has to find SMs while this (persistent, SM-filling) kernel runs, or it
@@ -1380,22 +1404,18 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     }
     uint32_t grid = sms * (uint32_t)ctx->agg_ctas_per_sm;
     if (grid > n_cols) grid = n_cols;
-    if (a->op != BMB200_OP_SHIFT_R_AND) p.dyn_bytes = (uint32_t)ctx->agg_dyn[a->op];
     if (ctx->agg_pipeline && ctx->gap_mode == 0 && set->n_gap_units && whole_set(a, set->v.n_vec) && flat_gap_set(ctx, set)) {
         // one AND-SUB group naming every vector once: a producer warp streams whole columns (agg_pipe_kernel), one CTA per SM.
         // OR stays on agg_kernel: its whole-set workloads measured at par or slower through the ring (DESIGN §3.1a)
         p.dyn_bytes = (uint32_t)ctx->pipe_dyn;
         const uint32_t pgrid = sms < n_cols ? sms : n_cols;
         agg_pipe_kernel<<<pgrid, kPipeThreads, ctx->pipe_dyn, ctx->stream>>>(p);
-    } else switch (a->op) {
-    case BMB200_OP_OR:      agg_kernel<BMB200_OP_OR><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_OR], ctx->stream>>>(p); break;
-    case BMB200_OP_AND:     agg_kernel<BMB200_OP_AND><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_AND], ctx->stream>>>(p); break;
-    case BMB200_OP_AND_SUB: agg_kernel<BMB200_OP_AND_SUB><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_AND_SUB], ctx->stream>>>(p); break;
-    case BMB200_OP_SHIFT_R_AND: shift_and_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p); break;
-    default:                agg_kernel<BMB200_OP_XOR><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_XOR], ctx->stream>>>(p); break;
+    } else if (a->op == BMB200_OP_SHIFT_R_AND) {
+        shift_and_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p);
+    } else {
+        launch_agg_kernel(ctx, a->op, grid, p);
     }
-    int rc = after_launch(ctx);
-    if (rc) { if (!*inout) bmb200_result_free(r); return rc; }
+    if ((rc = after_launch(ctx))) return bail(rc);
     *inout = r;
     if (store && compress) r->gaps_ready = true;      // bit -> GAP conversion is fused into the kernel epilogue
     return BMB200_OK;
@@ -1434,19 +1454,9 @@ int bmb200_binop(bmb200_ctx* ctx, const bmb200_set* set, int op, uint32_t va, ui
     // the two member ids (a, b) -> device, through the pinned group staging buffer like every aggregate
     const uint32_t mem[2] = {va, vb};
     const uint32_t off[3] = {0u, op == BMB200_OP_SUB ? 1u : 2u, 2u};
-    const size_t nwords = 5;
-    if (nwords > ctx->group_cap) {
-        cudaStreamSynchronize(ctx->stream);
-        cudaFree(ctx->d_group); if (ctx->h_group) cudaFreeHost(ctx->h_group);
-        ctx->d_group = nullptr; ctx->h_group = nullptr; ctx->group_cap = 0; ctx->last_group.clear();
-        if (cudaMalloc((void**)&ctx->d_group, 1024 * 4) != cudaSuccess || cudaMallocHost((void**)&ctx->h_group, 1024 * 4) != cudaSuccess) { ctx->last_err = "group buffer allocation"; return bail(BMB200_ERR_BADALLOC); }
-        ctx->group_cap = 1024;
-    }
-    ctx->last_group.clear();
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);              // the staging buffer may still feed a previous launch
-    memcpy(ctx->h_group, mem, 8); memcpy(ctx->h_group + 2, off, 12);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(ctx->d_group, ctx->h_group, nwords * 4, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
+    int rc = stage_group(ctx, mem, 2, off, 3, false);
+    if (rc) return bail(rc);
+    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
     if (e == cudaSuccess) set_agg_attrs(ctx, &e);
     if (e == cudaSuccess && !ctx->merge_attr_set) { e = cudaFuncSetAttribute(gap_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMergeSmem); ctx->merge_attr_set = (e == cudaSuccess); }
@@ -1458,24 +1468,12 @@ int bmb200_binop(bmb200_ctx* ctx, const bmb200_set* set, int op, uint32_t va, ui
     mp.kind = r->kind; mp.popcnt = r->popcnt; mp.digest = r->digest; mp.nruns = r->nruns; mp.gaps = r->gaps; mp.total = r->total;
     uint32_t mgrid = (cols + kMergeWarps - 1) / kMergeWarps; const uint32_t mmax = (uint32_t)ctx->sm_count * 8u; if (mgrid > mmax) mgrid = mmax;
     gap_merge_kernel<<<mgrid, kMergeWarps * 32, kMergeSmem, ctx->stream>>>(mp);
-    int rc = after_launch(ctx);
-    if (rc) return bail(rc);
+    if ((rc = after_launch(ctx))) return bail(rc);
     // 2) every other pairing (and merged blocks that outgrew the GAP format) through the block kernel, kinds by binop_rule
-    AggParams p{};
-    p.set = set->v; p.group = ctx->d_group; p.goff = ctx->d_group + 2; p.n_groups = 1;
-    p.nb_from = nb_from; p.n_cols = cols; p.compress = compress ? 1u : 0u; p.store_blocks = 1u;
-    p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
-    p.total = r->total; p.work_counter = ctx->d_work; p.or_blocks = nullptr;
-    p.gap_mode = (uint32_t)ctx->gap_mode; p.gap_pool_bytes = set->gap_pool_bytes; p.binary = 1u + bop;
+    AggParams p = agg_params(ctx, set, r, nb_from, cols, compress, true);
+    p.group = ctx->d_group; p.goff = ctx->d_group + 2; p.n_groups = 1; p.binary = 1u + bop;
     uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm); if (grid > cols) grid = cols;
-    const int kop = op == BMB200_OP_SUB ? BMB200_OP_AND_SUB : op;
-    p.dyn_bytes = (uint32_t)ctx->agg_dyn[kop];
-    switch (kop) {
-    case BMB200_OP_OR:      agg_kernel<BMB200_OP_OR><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_OR], ctx->stream>>>(p); break;
-    case BMB200_OP_AND:     agg_kernel<BMB200_OP_AND><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_AND], ctx->stream>>>(p); break;
-    case BMB200_OP_AND_SUB: agg_kernel<BMB200_OP_AND_SUB><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_AND_SUB], ctx->stream>>>(p); break;
-    default:                agg_kernel<BMB200_OP_XOR><<<grid, kAggThreads, ctx->agg_dyn[BMB200_OP_XOR], ctx->stream>>>(p); break;
-    }
+    launch_agg_kernel(ctx, op == BMB200_OP_SUB ? BMB200_OP_AND_SUB : op, grid, p);
     if ((rc = after_launch(ctx))) return bail(rc);
     *inout = r;
     return BMB200_OK;
@@ -1506,33 +1504,20 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
         int rc = result_alloc(ctx, n_cols, nv, store, store && compress, false, &r);
         if (rc) return rc;
     }
+    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
     r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
 
     // search values -> device through the (pinned) group staging buffer, 2 words per value
-    const size_t nvals = (size_t)nv * (a->pred == BMB200_SCAN_RANGE ? 2 : 1), nwords = 2 * nvals;
-    if (nwords > ctx->group_cap) {
-        cudaStreamSynchronize(ctx->stream);
-        cudaFree(ctx->d_group); if (ctx->h_group) cudaFreeHost(ctx->h_group);
-        ctx->d_group = nullptr; ctx->h_group = nullptr; ctx->group_cap = 0;
-        size_t cap = nwords < 1024 ? 1024 : nwords;
-        if (cudaMalloc((void**)&ctx->d_group, cap * 4) != cudaSuccess || cudaMallocHost((void**)&ctx->h_group, cap * 4) != cudaSuccess) {
-            ctx->last_err = "group buffer allocation"; if (!*inout) bmb200_result_free(r); return BMB200_ERR_BADALLOC;
-        }
-        ctx->group_cap = cap;
-    }
-    ctx->last_group.clear();                   // the buffer no longer holds aggregate member ids
-    cudaStreamSynchronize(ctx->stream);        // the staging buffer may still feed a previous launch
-    memcpy(ctx->h_group, a->values, nvals * 8);
-    CU(cudaMemcpyAsync(ctx->d_group, ctx->h_group, nvals * 8, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream));
-    CU(cudaMemsetAsync(r->total, 0, 8 * (size_t)nv, ctx->stream));
+    const size_t nvals = (size_t)nv * (a->pred == BMB200_SCAN_RANGE ? 2 : 1);
+    int rc = stage_group(ctx, reinterpret_cast<const uint32_t*>(a->values), 2 * nvals, nullptr, 0, false);
+    if (rc) return bail(rc);
+    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8 * (size_t)nv, ctx->stream);
+    if (e != cudaSuccess) { ctx->last_err = std::string("scan: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
 
     ScanParams sp{};
-    AggParams& p = sp.out;
-    p.set = set->v; p.n_groups = nv; p.nb_from = a->nb_from; p.n_cols = cols;
-    p.compress = compress ? 1u : 0u; p.store_blocks = store ? 1u : 0u;
-    p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
-    p.total = r->total; p.work_counter = ctx->d_work; p.or_blocks = nullptr;
+    sp.out = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
+    sp.out.n_groups = nv;
     sp.plane0 = a->plane0; sp.n_planes = a->n_planes; sp.universe = a->universe; sp.pred = (uint32_t)a->pred;
     sp.values = reinterpret_cast<const uint64_t*>(ctx->d_group);
     // values per pass: find_eq keeps one state per value (4 values share a pass), the inequalities two (2 values), RANGE four (2 values);
@@ -1547,8 +1532,7 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
     else if (mode == 1) { if (vg == 2) BMB200_SCAN_LAUNCH(2, 1); else BMB200_SCAN_LAUNCH(1, 1); }
     else                { if (vg == 2) BMB200_SCAN_LAUNCH(2, 2); else BMB200_SCAN_LAUNCH(1, 2); }
     #undef BMB200_SCAN_LAUNCH
-    int rc = after_launch(ctx);
-    if (rc) { if (!*inout) bmb200_result_free(r); return rc; }
+    if ((rc = after_launch(ctx))) return bail(rc);
     *inout = r;
     if (store && compress) r->gaps_ready = true;
     return BMB200_OK;
