@@ -40,11 +40,11 @@ SYMBOLS = [
     "bmb200_exchange_popcounts", "bmb200_exchange_fence", "bmb200_exchange_fetch", "bmb200_ctx_trim", "bmb200_binop",
     "bmb200_set_upload_slabs", "bmb200_host_slabs_prefetch", "bmb200_host_slab_alloc", "bmb200_host_slab_free",
     "bmb200_result_fetch_view_async", "bmb200_result_fetch_wait", "bmb200_exchange_mode",
-    "bmb200_result_fetch_column",
+    "bmb200_result_fetch_column", "bmb200_set_run_lists",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
-TUNE_GAP_MODE, TUNE_CTAS_PER_SM, TUNE_HOST_THREADS, TUNE_AGG_PIPELINE = 0, 1, 2, 3
+TUNE_GAP_MODE, TUNE_CTAS_PER_SM, TUNE_HOST_THREADS, TUNE_AGG_PIPELINE, TUNE_RUN_LISTS = 0, 1, 2, 3, 4
 
 
 class PackedSetC(C.Structure):
@@ -405,6 +405,12 @@ class DeviceSet:
         c = PackedSetC()
         self.ctx.check(lib().bmb200_set_device_ptrs(self._h, C.byref(c)), "set_device_ptrs")
         return c
+
+    def run_list_bytes(self) -> tuple[int, int]:
+        """(singles, long runs) bytes of the set's run-list companion; (0, 0) while none is built (TUNE_RUN_LISTS)."""
+        a, b = C.c_uint64(0), C.c_uint64(0)
+        self.ctx.check(lib().bmb200_set_run_lists(self._h, C.byref(a), C.byref(b)), "set_run_lists")
+        return a.value, b.value
 
     def stored_bytes(self) -> int:
         """Algorithmic source bytes: 8192 per bit-block + the 16-byte units of the GAP blocks."""

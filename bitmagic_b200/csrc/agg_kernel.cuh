@@ -302,25 +302,54 @@ __device__ __forceinline__ void flat_quad(uint32_t Ls, const uint4& q)
     if (reach > 32u) flat_quad_tail(Ls, q);
 }
 
+// Singles of the run-list companion (runlist_kernel.cuh): eight u16 bit positions per 128-bit load, one bit each.
+// MODE 0: one atomic per position.  MODE 1: test-first, as in flat_quad.
+template <int MODE>
+__device__ __forceinline__ void sgl_oct(uint32_t Ls, const uint4& q)
+{
+    const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+    uint32_t a[8], m[8];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        a[2 * i]     = and_or(w[i] >> 3, 0x1ffcu, Ls);  m[2 * i]     = 1u << (w[i] & 31u);
+        a[2 * i + 1] = and_or(w[i] >> 19, 0x1ffcu, Ls); m[2 * i + 1] = 1u << ((w[i] >> 16) & 31u);
+    }
+    if (MODE) {
+        uint32_t v[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = lds32(a[i]) & m[i];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) reds_and_if(a[i], ~m[i], v[i]);
+    } else {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) reds_and(a[i], ~m[i]);
+    }
+}
+
 // One slot of the FLAT window (bytes = what the bulk copy delivered, a multiple of 16; src = slot address + lane * 16): every lane eats
 // 4 runs per 128-bit load, 1 KB of the slot per step.  Deliberately ONE out-of-line copy per kernel: inlined into both slot
 // branches of the consumer (and unrolled) the sweep alone was ~50 KB of SASS, more than the instruction cache of an SM
-// sub-partition holds -- ncu showed `no_instruction` as the top stall of the GAP phase.
-template <int MODE>
+// sub-partition holds -- ncu showed `no_instruction` as the top stall of the GAP phase.  SGL: the stage holds companion singles.
+template <int MODE, bool SGL = false>
 __device__ __forceinline__ void flat_sweep_mode(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off)
 {
+    auto eat = [&](const uint4& q) { if (SGL) sgl_oct<MODE>(Ls, q); else flat_quad<MODE>(Ls, q); };
     uint32_t h = 0;
 #pragma unroll 1
     for (; h + 1024u <= bytes; h += 1024u) {
         const uint4 qa = lds128(src + h), qb = lds128(src + h + 512u);
-        flat_quad<MODE>(Ls, qa); flat_quad<MODE>(Ls, qb);
+        eat(qa); eat(qb);
     }
-    if (h + lane_off < bytes)        { const uint4 qa = lds128(src + h);        flat_quad<MODE>(Ls, qa); }     // last, partial KB of the window
-    if (h + 512u + lane_off < bytes) { const uint4 qb = lds128(src + h + 512u); flat_quad<MODE>(Ls, qb); }
+    if (h + lane_off < bytes)        { const uint4 qa = lds128(src + h);        eat(qa); }     // last, partial KB of the window
+    if (h + 512u + lane_off < bytes) { const uint4 qb = lds128(src + h + 512u); eat(qb); }
 }
 __device__ __noinline__ void flat_sweep_fn(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off, uint32_t mode)
 {
     if (mode) flat_sweep_mode<1>(Ls, src, bytes, lane_off); else flat_sweep_mode<0>(Ls, src, bytes, lane_off);
+}
+__device__ __noinline__ void sgl_sweep_fn(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off, uint32_t mode)
+{
+    if (mode) flat_sweep_mode<1, true>(Ls, src, bytes, lane_off); else flat_sweep_mode<0, true>(Ls, src, bytes, lane_off);
 }
 // The sweep's form for one column, re-sampled before each piece until it switches (warp-uniform): a 1024-bit sample of L (piece
 // number c varies the sample); below 25 % alive the test-first form wins (one shared load, rarely an atomic).  Bits of L only ever
@@ -970,7 +999,8 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
 // per stage) and HBM keeps ~kPipeStages x 8 KB per SM in flight across column boundaries, while 16 consumer warps classify the
 // column from its descriptor row, fold the staged bit-blocks (stage j = bit-block j of the segment) and sweep the staged GAP segment
 // in FLAT form.  A column whose GAP blocks are not all FLAT SUB-group blocks (raw GAP form, GAP blocks in the AND group) releases
-// its GAP stages unread and applies its GAP blocks straight from global memory.
+// its GAP stages unread and applies its GAP blocks straight from global memory.  With the run-list companion (RunLists, passed only
+// when the AND group holds no GAP block) the producer streams the column's companion singles and long runs in place of its GAP segment.
 // Protocol (no wait can outlive the producer): the producer claims a column only when a queue slot is free, publishes (item, #bit
 // stages, GAP bytes, first stage) and then issues all of the column's stages in order, each after its empty barrier; after the last
 // column it publishes an end marker.  Consumers read every queue entry, wait for exactly the stages the entry announces and release
@@ -997,7 +1027,16 @@ __global__ void desc_flat_check_kernel(const uint32_t* __restrict__ desc, size_t
     }
 }
 
-__global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggParams p)
+// The run-list companion of the set's GAP blocks (runlist_kernel.cuh), or all null.  The host passes it only when no GAP block of
+// the set belongs to the AND group; the kernel then streams each column's two companion parts in place of its GAP segment.
+struct RunLists {
+    const uint64_t* sgl_base;   // [n_blocks+1] 16-byte units of sgl
+    const uint64_t* lr_base;    // [n_blocks+1] 16-byte units of lr
+    const uint16_t* sgl;        // singles: u16 bit positions
+    const uint32_t* lr;         // long runs: FLAT pairs
+};
+
+__global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggParams p, const RunLists rl)
 {
     constexpr int OP = BMB200_OP_AND_SUB;
     extern __shared__ __align__(128) uint8_t dyn_smem[];
@@ -1008,7 +1047,8 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
     uint8_t* ring = dyn_smem + k_off + kLiveAlign;
 
     __shared__ __align__(8) uint64_t s_full[kPipeStages], s_empty[kPipeStages], s_qfull[kPipeQueue], s_qempty[kPipeQueue];
-    __shared__ uint4 s_q[kPipeQueue];                       // (item | ~0 = end, bit stages, GAP bytes, first stage)
+    __shared__ uint4 s_q[kPipeQueue];                       // (item | ~0 = end, bit stages, GAP or companion singles bytes, first stage)
+    __shared__ uint32_t s_qlr[kPipeQueue];                  // companion long-run bytes (0 without the companion)
     __shared__ uint32_t s_g1[kPipeMaxVec / 32];             // vector -> member of group1 (AND-SUB)
     __shared__ uint32_t s_brole[2][kPipeMaxVec / 32];       // bit-block j of the column -> group1, one buffer per column parity
     __shared__ uint32_t s_st[2][6];                         // flags, bit0, gap0, AND-group GAP blocks, non-FLAT, first GAP unit
@@ -1038,18 +1078,31 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
             const uint32_t item = atomicAdd(p.work_counter, 1u);
             if (item >= p.n_cols) { s_q[qs] = make_uint4(~0u, 0u, 0u, 0u); mbar_arrive(&s_qfull[qs]); return; }
             const uint32_t nb = p.nb_from + item;
-            const uint64_t b0 = p.set.bit_base[nb], g0 = p.set.gap_base[nb];
-            const uint32_t nbit = (uint32_t)(p.set.bit_base[nb + 1] - b0), gbytes = (uint32_t)((p.set.gap_base[nb + 1] - g0) * 16u);
-            s_q[qs] = make_uint4(item, nbit, gbytes, seq);
+            const uint64_t b0 = p.set.bit_base[nb];
+            const uint32_t nbit = (uint32_t)(p.set.bit_base[nb + 1] - b0);
+            // behind the bit-blocks: the GAP segment (gsrc, gbytes), or the companion's singles (gsrc, gbytes) and long runs (lsrc, lbytes)
+            uint32_t gbytes, lbytes = 0;
+            const uint8_t *gsrc, *lsrc = nullptr;
+            if (rl.sgl_base) {
+                const uint64_t s0 = rl.sgl_base[nb], l0 = rl.lr_base[nb];
+                gbytes = (uint32_t)((rl.sgl_base[nb + 1] - s0) * 16u); lbytes = (uint32_t)((rl.lr_base[nb + 1] - l0) * 16u);
+                gsrc = reinterpret_cast<const uint8_t*>(rl.sgl + s0 * 8u); lsrc = reinterpret_cast<const uint8_t*>(rl.lr + l0 * 4u);
+            } else {
+                const uint64_t g0 = p.set.gap_base[nb];
+                gbytes = (uint32_t)((p.set.gap_base[nb + 1] - g0) * 16u);
+                gsrc = reinterpret_cast<const uint8_t*>(p.set.gap_pool + g0 * kGapUnit);
+            }
+            s_q[qs] = make_uint4(item, nbit, gbytes, seq); s_qlr[qs] = lbytes;
             mbar_arrive(&s_qfull[qs]);
             const uint8_t* bsrc = reinterpret_cast<const uint8_t*>(p.set.bit_pool + b0 * kBlockWords);
-            const uint8_t* gsrc = reinterpret_cast<const uint8_t*>(p.set.gap_pool + g0 * kGapUnit);
-            const uint32_t ns = nbit + (gbytes + kPipeStage - 1u) / kPipeStage;
+            const uint32_t ng = nbit + (gbytes + kPipeStage - 1u) / kPipeStage, ns = ng + (lbytes + kPipeStage - 1u) / kPipeStage;
             for (uint32_t j = 0; j < ns; ++j, ++seq) {
                 const uint32_t s = seq % kPipeStages;
                 mbar_wait(&s_empty[s], ((seq / kPipeStages) & 1u) ^ 1u);
-                const uint32_t bytes = j < nbit ? kPipeStage : min(kPipeStage, gbytes - (j - nbit) * kPipeStage);
-                const uint8_t* src = j < nbit ? bsrc + (size_t)j * kPipeStage : gsrc + (size_t)(j - nbit) * kPipeStage;
+                uint32_t bytes; const uint8_t* src;
+                if (j < nbit)    { bytes = kPipeStage; src = bsrc + (size_t)j * kPipeStage; }
+                else if (j < ng) { const uint32_t o = (j - nbit) * kPipeStage; bytes = min(kPipeStage, gbytes - o); src = gsrc + o; }
+                else             { const uint32_t o = (j - ng) * kPipeStage;   bytes = min(kPipeStage, lbytes - o); src = lsrc + o; }
                 mbar_arrive_expect_tx(&s_full[s], bytes);
                 bulk_g2s(ring + (size_t)s * kPipeStage, src, bytes, &s_full[s]);
             }
@@ -1068,6 +1121,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
         if (tid < (int)(kPipeMaxVec / 32)) s_brole[b ^ 1u][tid] = 0u;
         mbar_wait(&s_qfull[qs], (qi / kPipeQueue) & 1u);
         const uint4 e = s_q[qs];
+        const uint32_t lbytes = s_qlr[qs];
         __syncwarp();
         if (lane == 0) mbar_arrive(&s_qempty[qs]);
         if (e.x == ~0u) break;
@@ -1143,7 +1197,22 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
 
         // ---- GAP phase: GAP stage g belongs to warp g % 16 ----
         const uint32_t ngs = (gbytes + kPipeStage - 1u) / kPipeStage;
-        if (flat) {
+        if (rl.sgl_base) {
+            // run-list companion: every GAP block is a SUB-group block, so the phase clears the column's singles (stages 0 .. ngs-1)
+            // and long runs (the stages behind them) from L; no lead-pad repair, no AND-group blocks
+            const uint32_t nst = ngs + (lbytes + kPipeStage - 1u) / kPipeStage;
+            uint32_t flat_mode = 0;
+            for (uint32_t g = (uint32_t)warp; g < nst; g += kAggWarps) {
+                const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
+                const uint32_t src = ring_s + s * kPipeStage + (uint32_t)lane * 16u;
+                mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
+                flat_update_mode(flat_mode, Ks, (uint32_t)lane, g);
+                if (g < ngs) sgl_sweep_fn(Ks, src, min(kPipeStage, gbytes - g * kPipeStage), (uint32_t)lane * 16u, flat_mode);
+                else         flat_sweep_fn(Ks, src, min(kPipeStage, lbytes - (g - ngs) * kPipeStage), (uint32_t)lane * 16u, flat_mode);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&s_empty[s], kAggWarps);
+            }
+        } else if (flat) {
             // a FLAT SUB-group block without lead pad starts with a 1-run whose pair slot holds the header: clear that whole run here
 #pragma unroll
             for (int i = 0; i < kPipePerThr; ++i) {

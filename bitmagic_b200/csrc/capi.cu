@@ -10,6 +10,7 @@
 
 #include "agg_kernel.cuh"
 #include "aux_kernels.cuh"
+#include "runlist_kernel.cuh"
 #include "scan_kernel.cuh"
 #include "shift_kernel.cuh"
 #include "binop_kernel.cuh"
@@ -53,6 +54,7 @@ struct bmb200_ctx {
     size_t agg_dyn[4] = {};                 // dynamic shared memory per agg_kernel<OP> (set_agg_attrs)
     size_t pipe_dyn = 0;                    // ... of agg_pipe_kernel
     int agg_pipeline = 1;                   // 1 = whole-set AND-SUB takes agg_pipe_kernel, 0 = always agg_kernel
+    int run_lists = 1;                      // run-list companion of agg_pipe_kernel: 0 never, 1 from a set's second qualifying call, 2 from its first
     int host_threads = 0;                   // host threads of bmb200_set_upload_vectors (0 = hardware concurrency, at most 64)
     uint8_t* h_ring[kStageSlots] = {};      // pinned staging ring of bmb200_set_upload_vectors (grow-only)
     size_t h_ring_cap = 0;
@@ -79,6 +81,14 @@ struct bmb200_set {
     uint64_t n_bit_blocks = 0, n_gap_units = 0;
     int flat_gaps = -1;                     // every GAP block in BMB200_DESC_GAP_FLAT form: 1 yes, 0 no, -1 not checked yet (flat_gap_set)
     uint64_t gap_pool_bytes = 0;            // readable bytes of gap_pool (with the allocation slack when owned)
+    std::vector<uint32_t> gap_vecs;         // bit v: vector v holds a GAP block in some column; empty until gap_vectors() asks
+    // run-list companion of the GAP blocks (runlist_kernel.cuh), always owned by the set and freed with it
+    int rl_state = 0;                       // 0 not built, 1 built, -1 cannot be built (device memory): calls run without it
+    uint32_t rl_calls = 0;                  // qualifying calls seen while not built
+    uint64_t *rl_sgl_base = nullptr, *rl_lr_base = nullptr;
+    uint16_t* rl_sgl = nullptr;
+    uint32_t* rl_lr = nullptr;
+    uint64_t rl_sgl_units = 0, rl_lr_units = 0;
     size_t cap_desc = 0, cap_base = 0, cap_bit = 0, cap_gap = 0;   // capacities when the arrays came from set_alloc (elements / blocks / units); 0 = not recyclable
 };
 
@@ -172,6 +182,12 @@ void free_set_arrays(bmb200_set* s)
     if (!s || !s->owns) return;
     cudaFree((void*)s->v.desc); cudaFree((void*)s->v.bit_base); cudaFree((void*)s->v.gap_base);
     cudaFree((void*)s->v.bit_pool); cudaFree((void*)s->v.gap_pool);
+}
+
+void free_run_lists(bmb200_set* s)
+{
+    cudaFree(s->rl_sgl_base); cudaFree(s->rl_lr_base); cudaFree(s->rl_sgl); cudaFree(s->rl_lr);
+    s->rl_sgl_base = s->rl_lr_base = nullptr; s->rl_sgl = nullptr; s->rl_lr = nullptr; s->rl_sgl_units = s->rl_lr_units = 0;
 }
 
 void free_result_arrays(bmb200_result* r)
@@ -424,6 +440,7 @@ int bmb200_ctx_set_tuning(bmb200_ctx* ctx, int key, int value)
     if (key == BMB200_TUNE_CTAS_PER_SM && value >= 1 && value <= kCtasPerSm) { ctx->agg_ctas_per_sm = value; return BMB200_OK; }
     if (key == BMB200_TUNE_HOST_THREADS && value >= 0 && value <= 64) { ctx->host_threads = value; return BMB200_OK; }
     if (key == BMB200_TUNE_AGG_PIPELINE && (value == 0 || value == 1)) { ctx->agg_pipeline = value; return BMB200_OK; }
+    if (key == BMB200_TUNE_RUN_LISTS && value >= 0 && value <= 2) { ctx->run_lists = value; return BMB200_OK; }
     return BMB200_ERR_BADARG;
 }
 
@@ -1115,6 +1132,7 @@ int bmb200_set_free(bmb200_set* s)
     bmb200_ctx* ctx = s->ctx;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
+    free_run_lists(s);                                       // derived data: never parked
     if (s->owns && s->cap_desc && !ctx->arena.full) {       // park the arrays for the next upload instead of cudaFree
         auto& a = ctx->arena;
         a.desc = (void*)s->v.desc; a.bb = (void*)s->v.bit_base; a.gb = (void*)s->v.gap_base; a.bp = (void*)s->v.bit_pool; a.gp = (void*)s->v.gap_pool;
@@ -1342,6 +1360,83 @@ static bool flat_gap_set(bmb200_ctx* ctx, const bmb200_set* set)
     return s->flat_gaps == 1;
 }
 
+// Which vectors hold a GAP block in some column: one pass over the descriptors and a wait for the answer, once per set.  Empty on failure.
+static const std::vector<uint32_t>& gap_vectors(bmb200_ctx* ctx, const bmb200_set* set)
+{
+    bmb200_set* s = const_cast<bmb200_set*>(set);
+    if (s->gap_vecs.empty()) {
+        const uint32_t M = set->v.n_vec, words = (M + 31u) / 32u;
+        std::vector<uint32_t> h(words, 0u);
+        uint32_t* d = nullptr;
+        const dim3 grid((M + 255u) / 256u, std::min(set->v.n_blocks, 256u));
+        bool ok = cudaMalloc((void**)&d, words * 4u) == cudaSuccess && cudaMemsetAsync(d, 0, words * 4u, ctx->stream) == cudaSuccess;
+        if (ok) { gap_vectors_kernel<<<grid, 256, 0, ctx->stream>>>(set->v.desc, M, set->v.n_blocks, d); ok = cudaGetLastError() == cudaSuccess; }
+        ok = ok && cudaMemcpyAsync(h.data(), d, words * 4u, cudaMemcpyDeviceToHost, ctx->stream) == cudaSuccess &&
+             cudaStreamSynchronize(ctx->stream) == cudaSuccess;
+        cudaFree(d);
+        if (ok) s->gap_vecs.swap(h); else cudaGetLastError();
+    }
+    return s->gap_vecs;
+}
+
+// Builds the run-list companion (runlist_kernel.cuh): count pass, scans, one wait to size the pools, write pass.  On any failure,
+// or when it would leave less than kRunListMargin of device memory free, the set is marked as having none (rl_state = -1).
+constexpr size_t kRunListMargin = size_t(1) << 30;
+static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
+{
+    const uint32_t nb = s->v.n_blocks;
+    cudaStream_t st = ctx->stream;
+    uint2* wcnt = nullptr; uint64_t *su = nullptr, *lu = nullptr;
+    uint64_t tails[2] = {0, 0};
+    bool ok = cudaMalloc((void**)&wcnt, (size_t)nb * kRlWarps * sizeof(uint2)) == cudaSuccess &&
+              cudaMalloc((void**)&su, (size_t)nb * 8) == cudaSuccess && cudaMalloc((void**)&lu, (size_t)nb * 8) == cudaSuccess &&
+              cudaMalloc((void**)&s->rl_sgl_base, ((size_t)nb + 1) * 8) == cudaSuccess &&
+              cudaMalloc((void**)&s->rl_lr_base, ((size_t)nb + 1) * 8) == cudaSuccess;
+    if (ok) {
+        rl_count_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wcnt, su, lu);
+        scan_u64_kernel<<<1, 1024, 0, st>>>(su, nb, s->rl_sgl_base);
+        scan_u64_kernel<<<1, 1024, 0, st>>>(lu, nb, s->rl_lr_base);
+        ok = cudaGetLastError() == cudaSuccess &&
+             cudaMemcpyAsync(&tails[0], s->rl_sgl_base + nb, 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaMemcpyAsync(&tails[1], s->rl_lr_base + nb, 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaStreamSynchronize(st) == cudaSuccess;
+    }
+    size_t free_b = 0, total_b = 0;
+    ok = ok && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b >= (tails[0] + tails[1]) * 16u + kRunListMargin &&
+         cudaMalloc((void**)&s->rl_sgl, std::max<uint64_t>(tails[0], 1u) * 16u) == cudaSuccess &&
+         cudaMalloc((void**)&s->rl_lr, std::max<uint64_t>(tails[1], 1u) * 16u) == cudaSuccess;
+    if (ok) {
+        rl_write_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wcnt, s->rl_sgl_base, s->rl_lr_base, s->rl_sgl, s->rl_lr);
+        ok = cudaGetLastError() == cudaSuccess && cudaStreamSynchronize(st) == cudaSuccess;
+    }
+    cudaFree(wcnt); cudaFree(su); cudaFree(lu);
+    if (!ok) { cudaGetLastError(); free_run_lists(s); s->rl_state = -1; return false; }
+    s->rl_sgl_units = tails[0]; s->rl_lr_units = tails[1]; s->rl_state = 1;
+    return true;
+}
+
+// agg_pipe_kernel streams the run-list companion in place of the GAP segments when no AND-group member holds a GAP block anywhere
+// in the set (then every GAP block is a 1-run source).  Builds it when due (ctx->run_lists); false = the call runs without it.
+static bool use_run_lists(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_batch_args* a, RunLists* rl)
+{
+    bmb200_set* s = const_cast<bmb200_set*>(set);
+    if (!ctx->run_lists || s->rl_state < 0) return false;
+    const std::vector<uint32_t>& gv = gap_vectors(ctx, set);
+    if (gv.empty()) return false;
+    for (uint32_t k = a->offsets[0]; k < a->offsets[1]; ++k)
+        if ((gv[a->members[k] >> 5] >> (a->members[k] & 31u)) & 1u) return false;
+    if (s->rl_state == 0 && (++s->rl_calls < (ctx->run_lists == 1 ? 2u : 1u) || !build_run_lists(ctx, s))) return false;
+    *rl = RunLists{s->rl_sgl_base, s->rl_lr_base, s->rl_sgl, s->rl_lr};
+    return true;
+}
+
+int bmb200_set_run_lists(const bmb200_set* s, uint64_t* sgl_bytes, uint64_t* lr_bytes)
+{
+    if (!s || !sgl_bytes || !lr_bytes) return BMB200_ERR_BADARG;
+    *sgl_bytes = s->rl_sgl_units * 16u; *lr_bytes = s->rl_lr_units * 16u;
+    return BMB200_OK;
+}
+
 int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_batch_args* a, bmb200_result** inout)
 {
     if (!ctx || !set || !a || !inout || set->ctx != ctx || !a->n_groups || !a->offsets) return BMB200_ERR_BADARG;
@@ -1404,12 +1499,15 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     }
     uint32_t grid = sms * (uint32_t)ctx->agg_ctas_per_sm;
     if (grid > n_cols) grid = n_cols;
-    if (ctx->agg_pipeline && ctx->gap_mode == 0 && set->n_gap_units && whole_set(a, set->v.n_vec) && flat_gap_set(ctx, set)) {
-        // one AND-SUB group naming every vector once: a producer warp streams whole columns (agg_pipe_kernel), one CTA per SM.
+    RunLists rl{};
+    if (ctx->agg_pipeline && ctx->gap_mode == 0 && set->n_gap_units && whole_set(a, set->v.n_vec) &&
+        (use_run_lists(ctx, set, a, &rl) || flat_gap_set(ctx, set))) {
+        // one AND-SUB group naming every vector once: a producer warp streams whole columns (agg_pipe_kernel), one CTA per SM,
+        // with the GAP segments or the run-list companion behind the bit-blocks.
         // OR stays on agg_kernel: its whole-set workloads measured at par or slower through the ring (DESIGN §3.1a)
         p.dyn_bytes = (uint32_t)ctx->pipe_dyn;
         const uint32_t pgrid = sms < n_cols ? sms : n_cols;
-        agg_pipe_kernel<<<pgrid, kPipeThreads, ctx->pipe_dyn, ctx->stream>>>(p);
+        agg_pipe_kernel<<<pgrid, kPipeThreads, ctx->pipe_dyn, ctx->stream>>>(p, rl);
     } else if (a->op == BMB200_OP_SHIFT_R_AND) {
         shift_and_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p);
     } else {

@@ -183,6 +183,8 @@ int bmb200_device_info(const bmb200_ctx* ctx, int* sm_count, int* cc_major, int*
 #define BMB200_TUNE_CTAS_PER_SM  1
 #define BMB200_TUNE_HOST_THREADS 2   /* host threads that pack blocks in bmb200_set_upload_vectors: 0 = all cores (at most 64) */
 #define BMB200_TUNE_AGG_PIPELINE 3   /* 1 (default) = whole-set AND-SUB aggregations take the streamed-column kernel, 0 = never (A/B reference) */
+#define BMB200_TUNE_RUN_LISTS    4   /* run-list companion of a set's GAP blocks, streamed by the whole-set AND-SUB kernel when the AND group
+                                        holds no GAP block: 1 (default) = built on the set's second such call, 2 = on its first, 0 = never */
 int bmb200_ctx_set_tuning(bmb200_ctx* ctx, int key, int value);
 /* pin the CALLING thread (and the threads it starts later, e.g. the packers of bmb200_set_upload_vectors) to the CPUs of the NUMA
  * node this context's GPU hangs off, so that pinned staging memory is allocated next to the GPU's PCIe root.  *node = the node, or
@@ -251,6 +253,9 @@ int bmb200_set_download(const bmb200_set* set, uint32_t nb_from, uint32_t nb_to,
 /* device addresses of the packed arrays (for torch / NCCL interop) */
 int bmb200_set_device_ptrs(const bmb200_set* set, bmb200_packed_set* out);
 int bmb200_set_free(bmb200_set* set);
+/* bytes of the set's run-list companion (BMB200_TUNE_RUN_LISTS): singles part and long-run part; 0 / 0 while none is built.
+ * It is freed with the set. */
+int bmb200_set_run_lists(const bmb200_set* set, uint64_t* sgl_bytes, uint64_t* lr_bytes);
 
 /* synthetic input generator (bench / test support): vector v has iid bit density
  * density[v], counter-based RNG keyed by seed[v]; with optimize != 0 every block is
