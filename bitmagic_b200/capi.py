@@ -40,7 +40,7 @@ SYMBOLS = [
     "bmb200_exchange_popcounts", "bmb200_exchange_fence", "bmb200_exchange_fetch", "bmb200_ctx_trim", "bmb200_binop",
     "bmb200_set_upload_slabs", "bmb200_host_slabs_prefetch", "bmb200_host_slab_alloc", "bmb200_host_slab_free",
     "bmb200_result_fetch_view_async", "bmb200_result_fetch_wait", "bmb200_exchange_mode",
-    "bmb200_result_fetch_column", "bmb200_set_run_lists",
+    "bmb200_result_fetch_column", "bmb200_set_run_lists", "bmb200_set_bit_run_lists",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
@@ -411,6 +411,13 @@ class DeviceSet:
         a, b = C.c_uint64(0), C.c_uint64(0)
         self.ctx.check(lib().bmb200_set_run_lists(self._h, C.byref(a), C.byref(b)), "set_run_lists")
         return a.value, b.value
+
+    def bit_run_list_bytes(self) -> tuple[int, int, int]:
+        """(singles, long runs) bytes of the companion's part B, the listed sparse bit-blocks, and how many blocks it lists;
+        (0, 0, 0) while none is built."""
+        a, b, n = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        self.ctx.check(lib().bmb200_set_bit_run_lists(self._h, C.byref(a), C.byref(b), C.byref(n)), "set_bit_run_lists")
+        return a.value, b.value, n.value
 
     def stored_bytes(self) -> int:
         """Algorithmic source bytes: 8192 per bit-block + the 16-byte units of the GAP blocks."""

@@ -1000,14 +1000,19 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
 // column from its descriptor row, fold the staged bit-blocks (stage j = bit-block j of the segment) and sweep the staged GAP segment
 // in FLAT form.  A column whose GAP blocks are not all FLAT SUB-group blocks (raw GAP form, GAP blocks in the AND group) releases
 // its GAP stages unread and applies its GAP blocks straight from global memory.  With the run-list companion (RunLists, passed only
-// when the AND group holds no GAP block) the producer streams the column's companion singles and long runs in place of its GAP segment.
+// when the AND group holds no GAP block) the producer streams the column's companion singles and long runs in place of its GAP segment:
+// part A (the GAP blocks' runs), or A + B (also the runs of the listed bit-blocks, which it then does not stream) when the AND group
+// holds no listed bit-block either.
 // Protocol (no wait can outlive the producer): the producer claims a column only when a queue slot is free, publishes (item, #bit
 // stages, GAP bytes, first stage) and then issues all of the column's stages in order, each after its empty barrier; after the last
 // column it publishes an end marker.  Consumers read every queue entry, wait for exactly the stages the entry announces and release
-// each of them exactly once (bit stage: every warp arrives; GAP stage: its one reader arrives for all 16).
-// Parity waits are only sound when the waiter has seen the stage's previous fill complete.  Bit stages are waited for by every
-// warp in order; GAP stage g goes to warp g % 16, so with a ring of a multiple of 16 stages the previous fill of each stage a warp
-// waits for was one of its own GAP stages, or a bit stage / an earlier column that every warp has finished.
+// each of them exactly once (bit stage: every warp arrives; GAP stage: its one reader arrives for all 16).  They free the queue slot
+// once the column is classified, because classification reads the column's listed flags that the producer staged with the entry.
+// With part B the entry's bit stages are the column's unlisted bit-blocks in order; stage j is the j-th of them.
+// Parity waits are only sound when the waiter has seen the stage's previous fill complete.  Bit stages (streamed ones only, with
+// part B) are still waited for by every warp in order; GAP or companion stage g still goes to warp g % 16, so with a ring of a
+// multiple of 16 stages the previous fill of each stage a warp waits for was one of its own GAP stages, or a bit stage / an earlier
+// column that every warp has finished.
 constexpr int      kPipeStages  = 16;                      // 128 KB of stages
 constexpr uint32_t kPipeStage   = 8192u;
 constexpr int      kPipeQueue   = 2;                       // columns claimed ahead of the consumers (more would unbalance the tail)
@@ -1027,14 +1032,19 @@ __global__ void desc_flat_check_kernel(const uint32_t* __restrict__ desc, size_t
     }
 }
 
-// The run-list companion of the set's GAP blocks (runlist_kernel.cuh), or all null.  The host passes it only when no GAP block of
-// the set belongs to the AND group; the kernel then streams each column's two companion parts in place of its GAP segment.
+// The run-list companion of the set's GAP blocks and sparse bit-blocks (runlist_kernel.cuh), or all null.  The host passes it only
+// when no GAP block of the set belongs to the AND group; the kernel then streams each column's singles and long runs in place of its
+// GAP segment: part A only (listed null), or A + B (listed set: then no listed bit-block belongs to the AND group either).
 struct RunLists {
     const uint64_t* sgl_base;   // [n_blocks+1] 16-byte units of sgl
     const uint64_t* lr_base;    // [n_blocks+1] 16-byte units of lr
+    const uint64_t* sgl_mid;    // [n_blocks] end of column nb's part A singles = start of its part B
+    const uint64_t* lr_mid;     // [n_blocks] ... long runs
     const uint16_t* sgl;        // singles: u16 bit positions
     const uint32_t* lr;         // long runs: FLAT pairs
+    const uint32_t* listed;     // bit i: bit-block i of bit_pool is in part B and not streamed; null = stream part A only
 };
+constexpr uint32_t kPipeLstWords = kPipeMaxVec / 32u;       // listed flags of one column's bit-blocks
 
 __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggParams p, const RunLists rl)
 {
@@ -1049,6 +1059,8 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
     __shared__ __align__(8) uint64_t s_full[kPipeStages], s_empty[kPipeStages], s_qfull[kPipeQueue], s_qempty[kPipeQueue];
     __shared__ uint4 s_q[kPipeQueue];                       // (item | ~0 = end, bit stages, GAP or companion singles bytes, first stage)
     __shared__ uint32_t s_qlr[kPipeQueue];                  // companion long-run bytes (0 without the companion)
+    __shared__ uint32_t s_lst[kPipeQueue][kPipeLstWords];   // with part B: bit j = the column's bit-block j is listed
+    __shared__ uint32_t s_lrk[kPipeQueue][kPipeLstWords];   // ... listed bit-blocks in words < w
     __shared__ uint32_t s_g1[kPipeMaxVec / 32];             // vector -> member of group1 (AND-SUB)
     __shared__ uint32_t s_brole[2][kPipeMaxVec / 32];       // bit-block j of the column -> group1, one buffer per column parity
     __shared__ uint32_t s_st[2][6];                         // flags, bit0, gap0, AND-group GAP blocks, non-FLAT, first GAP unit
@@ -1081,27 +1093,43 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
             const uint64_t b0 = p.set.bit_base[nb];
             const uint32_t nbit = (uint32_t)(p.set.bit_base[nb + 1] - b0);
             // behind the bit-blocks: the GAP segment (gsrc, gbytes), or the companion's singles (gsrc, gbytes) and long runs (lsrc, lbytes)
-            uint32_t gbytes, lbytes = 0;
+            uint32_t gbytes, lbytes = 0, nlst = 0;
             const uint8_t *gsrc, *lsrc = nullptr;
             if (rl.sgl_base) {
                 const uint64_t s0 = rl.sgl_base[nb], l0 = rl.lr_base[nb];
-                gbytes = (uint32_t)((rl.sgl_base[nb + 1] - s0) * 16u); lbytes = (uint32_t)((rl.lr_base[nb + 1] - l0) * 16u);
+                const uint64_t s1 = rl.listed ? rl.sgl_base[nb + 1] : rl.sgl_mid[nb], l1 = rl.listed ? rl.lr_base[nb + 1] : rl.lr_mid[nb];
+                gbytes = (uint32_t)((s1 - s0) * 16u); lbytes = (uint32_t)((l1 - l0) * 16u);
                 gsrc = reinterpret_cast<const uint8_t*>(rl.sgl + s0 * 8u); lsrc = reinterpret_cast<const uint8_t*>(rl.lr + l0 * 4u);
+                if (rl.listed) {        // stage the column's listed flags (bit j = bit-block j) and their running counts for everyone
+                    const uint32_t* lw = rl.listed + (b0 >> 5);
+                    const uint32_t sh = (uint32_t)b0 & 31u, nw = (nbit + 31u) / 32u;
+                    uint32_t r = lw[0];
+#pragma unroll 4
+                    for (uint32_t w = 0; w < nw; ++w) {
+                        const uint32_t r1 = lw[w + 1u];
+                        uint32_t f = __funnelshift_r(r, r1, sh);
+                        if (32u * w + 32u > nbit) f &= (1u << (nbit & 31u)) - 1u;
+                        s_lst[qs][w] = f; s_lrk[qs][w] = nlst; nlst += __popc(f); r = r1;
+                    }
+                }
             } else {
                 const uint64_t g0 = p.set.gap_base[nb];
                 gbytes = (uint32_t)((p.set.gap_base[nb + 1] - g0) * 16u);
                 gsrc = reinterpret_cast<const uint8_t*>(p.set.gap_pool + g0 * kGapUnit);
             }
-            s_q[qs] = make_uint4(item, nbit, gbytes, seq); s_qlr[qs] = lbytes;
+            const uint32_t nstr = nbit - nlst;                   // streamed bit-blocks
+            s_q[qs] = make_uint4(item, nstr, gbytes, seq); s_qlr[qs] = lbytes;
             mbar_arrive(&s_qfull[qs]);
             const uint8_t* bsrc = reinterpret_cast<const uint8_t*>(p.set.bit_pool + b0 * kBlockWords);
-            const uint32_t ng = nbit + (gbytes + kPipeStage - 1u) / kPipeStage, ns = ng + (lbytes + kPipeStage - 1u) / kPipeStage;
-            for (uint32_t j = 0; j < ns; ++j, ++seq) {
+            const uint32_t ng = nstr + (gbytes + kPipeStage - 1u) / kPipeStage, ns = ng + (lbytes + kPipeStage - 1u) / kPipeStage;
+            for (uint32_t j = 0, jb = 0; j < ns; ++j, ++seq) {
                 const uint32_t s = seq % kPipeStages;
+                if (j < nstr && nlst)                            // the next unlisted bit-block
+                    while ((s_lst[qs][jb >> 5] >> (jb & 31u)) & 1u) ++jb;
                 mbar_wait(&s_empty[s], ((seq / kPipeStages) & 1u) ^ 1u);
                 uint32_t bytes; const uint8_t* src;
-                if (j < nbit)    { bytes = kPipeStage; src = bsrc + (size_t)j * kPipeStage; }
-                else if (j < ng) { const uint32_t o = (j - nbit) * kPipeStage; bytes = min(kPipeStage, gbytes - o); src = gsrc + o; }
+                if (j < nstr)    { bytes = kPipeStage; src = bsrc + (size_t)jb++ * kPipeStage; }
+                else if (j < ng) { const uint32_t o = (j - nstr) * kPipeStage; bytes = min(kPipeStage, gbytes - o); src = gsrc + o; }
                 else             { const uint32_t o = (j - ng) * kPipeStage;   bytes = min(kPipeStage, lbytes - o); src = lsrc + o; }
                 mbar_arrive_expect_tx(&s_full[s], bytes);
                 bulk_g2s(ring + (size_t)s * kPipeStage, src, bytes, &s_full[s]);
@@ -1122,8 +1150,6 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
         mbar_wait(&s_qfull[qs], (qi / kPipeQueue) & 1u);
         const uint4 e = s_q[qs];
         const uint32_t lbytes = s_qlr[qs];
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&s_qempty[qs]);
         if (e.x == ~0u) break;
         const uint32_t item = e.x, nbit = e.y, gbytes = e.z, seq0 = e.w;
         const uint32_t nb = p.nb_from + item;
@@ -1145,7 +1171,18 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
             const uint32_t d = dv[i], kind = d & 3u;
             const bool g1 = (s_g1[v >> 5] >> (v & 31u)) & 1u;
             if (kind == BMB200_BLK_BIT) {
-                if (g1) atomicOr(&s_brole[b][((d >> 2) & (kPipeMaxVec - 1u)) >> 5], 1u << ((d >> 2) & 31u)); else ++nb0;
+                // role by streamed index: rel minus the listed blocks below it (a listed block is a SUB-group block, never streamed)
+                if (g1) {
+                    uint32_t j = (d >> 2) & (kPipeMaxVec - 1u);
+                    if (rl.listed) {
+                        const uint32_t f = s_lst[qs][j >> 5], below = f & ((1u << (j & 31u)) - 1u);
+                        if ((f >> (j & 31u)) & 1u) continue;
+                        j -= s_lrk[qs][j >> 5] + __popc(below);
+                    }
+                    atomicOr(&s_brole[b][j >> 5], 1u << (j & 31u));
+                } else {
+                    ++nb0;
+                }
             } else if (kind == BMB200_BLK_GAP) {
                 const uint32_t u = (d >> 2) & kRelMask;
                 if (g1) {
@@ -1173,6 +1210,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
             if (lo != ~0u) atomicMin(&s_st[b][5], lo);
         }
         agg_sync<true>();
+        if (lane == 0) mbar_arrive(&s_qempty[qs]);               // the entry and its listed flags are read: the slot may be refilled
         // FLAT: the whole GAP segment is a flat window of 1-run sources (headers, pads and tail fill decode to empty runs)
         const bool flat = s_st[b][4] == 0u && s_st[b][5] == 0u;
         const uint32_t nag = s_st[b][3];                         // <= kPipeMaxAndGap when flat

@@ -85,10 +85,13 @@ struct bmb200_set {
     // run-list companion of the GAP blocks (runlist_kernel.cuh), always owned by the set and freed with it
     int rl_state = 0;                       // 0 not built, 1 built, -1 cannot be built (device memory): calls run without it
     uint32_t rl_calls = 0;                  // qualifying calls seen while not built
-    uint64_t *rl_sgl_base = nullptr, *rl_lr_base = nullptr;
+    uint64_t *rl_sgl_base = nullptr, *rl_lr_base = nullptr, *rl_sgl_mid = nullptr, *rl_lr_mid = nullptr;
     uint16_t* rl_sgl = nullptr;
     uint32_t* rl_lr = nullptr;
-    uint64_t rl_sgl_units = 0, rl_lr_units = 0;
+    uint32_t* rl_listed = nullptr;          // bit i: bit-block i of bit_pool is listed in part B
+    uint64_t rl_sgl_units = 0, rl_lr_units = 0;        // part A
+    uint64_t rl_b_sgl_units = 0, rl_b_lr_units = 0, rl_listed_blocks = 0;   // part B
+    std::vector<uint32_t> listed_vecs;      // bit v: vector v holds a listed bit-block in some column (set with the companion)
     size_t cap_desc = 0, cap_base = 0, cap_bit = 0, cap_gap = 0;   // capacities when the arrays came from set_alloc (elements / blocks / units); 0 = not recyclable
 };
 
@@ -186,8 +189,11 @@ void free_set_arrays(bmb200_set* s)
 
 void free_run_lists(bmb200_set* s)
 {
-    cudaFree(s->rl_sgl_base); cudaFree(s->rl_lr_base); cudaFree(s->rl_sgl); cudaFree(s->rl_lr);
-    s->rl_sgl_base = s->rl_lr_base = nullptr; s->rl_sgl = nullptr; s->rl_lr = nullptr; s->rl_sgl_units = s->rl_lr_units = 0;
+    cudaFree(s->rl_sgl_base); cudaFree(s->rl_lr_base); cudaFree(s->rl_sgl_mid); cudaFree(s->rl_lr_mid);
+    cudaFree(s->rl_sgl); cudaFree(s->rl_lr); cudaFree(s->rl_listed);
+    s->rl_sgl_base = s->rl_lr_base = s->rl_sgl_mid = s->rl_lr_mid = nullptr; s->rl_sgl = nullptr; s->rl_lr = nullptr; s->rl_listed = nullptr;
+    s->rl_sgl_units = s->rl_lr_units = s->rl_b_sgl_units = s->rl_b_lr_units = s->rl_listed_blocks = 0;
+    s->listed_vecs.clear();
 }
 
 void free_result_arrays(bmb200_result* r)
@@ -1379,44 +1385,58 @@ static const std::vector<uint32_t>& gap_vectors(bmb200_ctx* ctx, const bmb200_se
     return s->gap_vecs;
 }
 
-// Builds the run-list companion (runlist_kernel.cuh): count pass, scans, one wait to size the pools, write pass.  On any failure,
-// or when it would leave less than kRunListMargin of device memory free, the set is marked as having none (rl_state = -1).
+// Builds the run-list companion (runlist_kernel.cuh): count pass (which also lists the sparse bit-blocks), scans, one wait to size
+// the pools, write pass, then which vectors hold a listed block.  On any failure, or when parts A + B would leave less than
+// kRunListMargin of device memory free, the set is marked as having none (rl_state = -1).
 constexpr size_t kRunListMargin = size_t(1) << 30;
 static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
 {
-    const uint32_t nb = s->v.n_blocks;
+    const uint32_t nb = s->v.n_blocks, M = s->v.n_vec, vwords = (M + 31u) / 32u;
+    const size_t lwords = (size_t)(s->n_bit_blocks + 31u) / 32u + 2u;   // + the word the kernel's funnel shift reads past a column
     cudaStream_t st = ctx->stream;
-    uint2* wcnt = nullptr; uint64_t *su = nullptr, *lu = nullptr;
-    uint64_t tails[2] = {0, 0};
-    bool ok = cudaMalloc((void**)&wcnt, (size_t)nb * kRlWarps * sizeof(uint2)) == cudaSuccess &&
+    uint2* wcnt = nullptr; uint64_t *su = nullptr, *lu = nullptr; unsigned long long* tot = nullptr; uint32_t* lv = nullptr;
+    uint64_t h_tot[5] = {0, 0, 0, 0, 0};
+    std::vector<uint32_t> h_lv(vwords, 0u);
+    bool ok = cudaMalloc((void**)&wcnt, (size_t)nb * 2 * kRlWarps * sizeof(uint2)) == cudaSuccess &&
               cudaMalloc((void**)&su, (size_t)nb * 8) == cudaSuccess && cudaMalloc((void**)&lu, (size_t)nb * 8) == cudaSuccess &&
+              cudaMalloc((void**)&tot, sizeof(h_tot)) == cudaSuccess && cudaMalloc((void**)&lv, vwords * 4u) == cudaSuccess &&
               cudaMalloc((void**)&s->rl_sgl_base, ((size_t)nb + 1) * 8) == cudaSuccess &&
-              cudaMalloc((void**)&s->rl_lr_base, ((size_t)nb + 1) * 8) == cudaSuccess;
+              cudaMalloc((void**)&s->rl_lr_base, ((size_t)nb + 1) * 8) == cudaSuccess &&
+              cudaMalloc((void**)&s->rl_sgl_mid, (size_t)nb * 8) == cudaSuccess && cudaMalloc((void**)&s->rl_lr_mid, (size_t)nb * 8) == cudaSuccess &&
+              cudaMalloc((void**)&s->rl_listed, lwords * 4u) == cudaSuccess &&
+              cudaMemsetAsync(s->rl_listed, 0, lwords * 4u, st) == cudaSuccess && cudaMemsetAsync(tot, 0, sizeof(h_tot), st) == cudaSuccess &&
+              cudaMemsetAsync(lv, 0, vwords * 4u, st) == cudaSuccess;
     if (ok) {
-        rl_count_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wcnt, su, lu);
+        rl_count_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wcnt, su, lu, s->rl_listed, tot);
         scan_u64_kernel<<<1, 1024, 0, st>>>(su, nb, s->rl_sgl_base);
         scan_u64_kernel<<<1, 1024, 0, st>>>(lu, nb, s->rl_lr_base);
-        ok = cudaGetLastError() == cudaSuccess &&
-             cudaMemcpyAsync(&tails[0], s->rl_sgl_base + nb, 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
-             cudaMemcpyAsync(&tails[1], s->rl_lr_base + nb, 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+        ok = cudaGetLastError() == cudaSuccess && cudaMemcpyAsync(h_tot, tot, sizeof(h_tot), cudaMemcpyDeviceToHost, st) == cudaSuccess &&
              cudaStreamSynchronize(st) == cudaSuccess;
     }
+    const uint64_t sgl_units = h_tot[0] + h_tot[2], lr_units = h_tot[1] + h_tot[3];
     size_t free_b = 0, total_b = 0;
-    ok = ok && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b >= (tails[0] + tails[1]) * 16u + kRunListMargin &&
-         cudaMalloc((void**)&s->rl_sgl, std::max<uint64_t>(tails[0], 1u) * 16u) == cudaSuccess &&
-         cudaMalloc((void**)&s->rl_lr, std::max<uint64_t>(tails[1], 1u) * 16u) == cudaSuccess;
+    ok = ok && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b >= (sgl_units + lr_units) * 16u + kRunListMargin &&
+         cudaMalloc((void**)&s->rl_sgl, std::max<uint64_t>(sgl_units, 1u) * 16u) == cudaSuccess &&
+         cudaMalloc((void**)&s->rl_lr, std::max<uint64_t>(lr_units, 1u) * 16u) == cudaSuccess;
     if (ok) {
-        rl_write_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wcnt, s->rl_sgl_base, s->rl_lr_base, s->rl_sgl, s->rl_lr);
-        ok = cudaGetLastError() == cudaSuccess && cudaStreamSynchronize(st) == cudaSuccess;
+        rl_write_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wcnt, s->rl_sgl_base, s->rl_lr_base, s->rl_listed, s->rl_sgl, s->rl_lr,
+                                                   s->rl_sgl_mid, s->rl_lr_mid);
+        const dim3 grid((M + 255u) / 256u, std::min(nb, 256u));
+        if (h_tot[4]) listed_vectors_kernel<<<grid, 256, 0, st>>>(s->v.desc, s->v.bit_base, s->rl_listed, M, nb, lv);
+        ok = cudaGetLastError() == cudaSuccess && cudaMemcpyAsync(h_lv.data(), lv, vwords * 4u, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaStreamSynchronize(st) == cudaSuccess;
     }
-    cudaFree(wcnt); cudaFree(su); cudaFree(lu);
+    cudaFree(wcnt); cudaFree(su); cudaFree(lu); cudaFree(tot); cudaFree(lv);
     if (!ok) { cudaGetLastError(); free_run_lists(s); s->rl_state = -1; return false; }
-    s->rl_sgl_units = tails[0]; s->rl_lr_units = tails[1]; s->rl_state = 1;
+    s->rl_sgl_units = h_tot[0]; s->rl_lr_units = h_tot[1];
+    s->rl_b_sgl_units = h_tot[2]; s->rl_b_lr_units = h_tot[3]; s->rl_listed_blocks = h_tot[4];
+    s->listed_vecs.swap(h_lv); s->rl_state = 1;
     return true;
 }
 
 // agg_pipe_kernel streams the run-list companion in place of the GAP segments when no AND-group member holds a GAP block anywhere
-// in the set (then every GAP block is a 1-run source).  Builds it when due (ctx->run_lists); false = the call runs without it.
+// in the set (then every GAP block is a 1-run source): part A, plus part B in place of the listed bit-blocks when no AND-group
+// member holds a listed block either.  Builds it when due (ctx->run_lists); false = the call runs without it.
 static bool use_run_lists(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_batch_args* a, RunLists* rl)
 {
     bmb200_set* s = const_cast<bmb200_set*>(set);
@@ -1426,7 +1446,10 @@ static bool use_run_lists(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_b
     for (uint32_t k = a->offsets[0]; k < a->offsets[1]; ++k)
         if ((gv[a->members[k] >> 5] >> (a->members[k] & 31u)) & 1u) return false;
     if (s->rl_state == 0 && (++s->rl_calls < (ctx->run_lists == 1 ? 2u : 1u) || !build_run_lists(ctx, s))) return false;
-    *rl = RunLists{s->rl_sgl_base, s->rl_lr_base, s->rl_sgl, s->rl_lr};
+    bool part_b = s->rl_listed_blocks != 0;
+    for (uint32_t k = a->offsets[0]; part_b && k < a->offsets[1]; ++k)
+        if ((s->listed_vecs[a->members[k] >> 5] >> (a->members[k] & 31u)) & 1u) part_b = false;
+    *rl = RunLists{s->rl_sgl_base, s->rl_lr_base, s->rl_sgl_mid, s->rl_lr_mid, s->rl_sgl, s->rl_lr, part_b ? s->rl_listed : nullptr};
     return true;
 }
 
@@ -1434,6 +1457,13 @@ int bmb200_set_run_lists(const bmb200_set* s, uint64_t* sgl_bytes, uint64_t* lr_
 {
     if (!s || !sgl_bytes || !lr_bytes) return BMB200_ERR_BADARG;
     *sgl_bytes = s->rl_sgl_units * 16u; *lr_bytes = s->rl_lr_units * 16u;
+    return BMB200_OK;
+}
+
+int bmb200_set_bit_run_lists(const bmb200_set* s, uint64_t* sgl_bytes, uint64_t* lr_bytes, uint64_t* listed_blocks)
+{
+    if (!s || !sgl_bytes || !lr_bytes || !listed_blocks) return BMB200_ERR_BADARG;
+    *sgl_bytes = s->rl_b_sgl_units * 16u; *lr_bytes = s->rl_b_lr_units * 16u; *listed_blocks = s->rl_listed_blocks;
     return BMB200_OK;
 }
 

@@ -256,6 +256,9 @@ int bmb200_set_free(bmb200_set* set);
 /* bytes of the set's run-list companion (BMB200_TUNE_RUN_LISTS): singles part and long-run part; 0 / 0 while none is built.
  * It is freed with the set. */
 int bmb200_set_run_lists(const bmb200_set* set, uint64_t* sgl_bytes, uint64_t* lr_bytes);
+/* part B of the companion: the listed runs of the set's sparse bit-blocks (singles and long-run bytes) and how many bit-blocks it
+ * lists; 0 / 0 / 0 while none is built.  bmb200_set_run_lists reports part A, the runs of the GAP blocks. */
+int bmb200_set_bit_run_lists(const bmb200_set* set, uint64_t* sgl_bytes, uint64_t* lr_bytes, uint64_t* listed_blocks);
 
 /* synthetic input generator (bench / test support): vector v has iid bit density
  * density[v], counter-based RNG keyed by seed[v]; with optimize != 0 every block is

@@ -1,7 +1,8 @@
 """C3's data through the whole-set AND-SUB kernel with the run-list companion (TUNE_RUN_LISTS 1) and without it (0), alternated,
-CUDA events over 20 calls, for an AND group of bit-block vectors ({1, 2}: the companion is used) and one with a GAP vector
-({1, 601}: it is not).  Prints ms per call, the bytes each launch streams next to bench.py's algorithmic bytes (which count the
-stored GAP blocks), the one-time build, popcount / digest equality, and the card it ran on.
+CUDA events over 20 calls, for an AND group of bit-block vectors ({1, 2}: parts A and B are used) and one with a GAP vector
+({1, 601}: the companion is not).  Prints ms per call, the bytes each launch streams (unlisted bit-blocks, the companion parts it
+reads, results) next to bench.py's algorithmic bytes (which count every stored block), part B's size and listed blocks, the
+one-time build, popcount / digest equality, and the card it ran on.
 python scripts/bench_run_lists.py   (from the repository root, on an H100)"""
 import json
 import subprocess
@@ -54,10 +55,16 @@ for g0 in ([0, 1], [0, 600]):
             res_bytes = int((k == bm.BLK_BIT).sum()) * 8192 + int(2 * (n[k == bm.BLK_GAP].astype(np.int64) + 1).sum())
             res.free()
     sgl, lr = dset.run_list_bytes()
+    bsgl, blr, listed = dset.bit_run_list_bytes()
     alg = counts["bit"] * 8192 + gap_words * 2 + res_bytes + n_cols * 12
-    streamed = counts["bit"] * 8192 + (sgl + lr if g0 == [0, 1] else dset.n_gap_units * 16) + res_bytes + n_cols * 12
+    if g0 == [0, 1]:          # A + B in place of the GAP segments and the listed bit-blocks
+        src = (counts["bit"] - listed) * 8192 + sgl + lr + bsgl + blr
+    else:
+        src = counts["bit"] * 8192 + dset.n_gap_units * 16
+    streamed = src + res_bytes + n_cols * 12
     out["same"] = out.pop("pop0") == out.pop("pop1") and out.pop("dig0") == out.pop("dig1")
     out["companion_bytes"] = {"singles": sgl, "long_runs": lr}
+    out["part_b"] = {"singles": bsgl, "long_runs": blr, "listed_blocks": listed, "listed_per_column": round(listed / n_cols, 2)}
     out["bench_algorithmic_bytes"] = alg
     out["streamed_bytes_mode1"] = streamed
     out["streamed_gbs_mode1"] = round(streamed / (min(out["ms_mode1"]) * 1e-3) / 1e9, 1)
