@@ -41,6 +41,7 @@ SYMBOLS = [
     "bmb200_set_upload_slabs", "bmb200_host_slabs_prefetch", "bmb200_host_slab_alloc", "bmb200_host_slab_free",
     "bmb200_result_fetch_view_async", "bmb200_result_fetch_wait", "bmb200_exchange_mode",
     "bmb200_result_fetch_column", "bmb200_set_run_lists", "bmb200_set_bit_run_lists",
+    "bmb200_rank_decompress", "bmb200_rank_compress",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
@@ -554,6 +555,28 @@ def scan(ctx: Context, dset: DeviceSet, pred: int, values, plane0: int, n_planes
     ctx.check(lib().bmb200_scan(ctx._h, dset._h, C.byref(args), C.byref(res._h)), "scan")
     res.n_cols = ((nb_to if nb_to else dset.n_blocks) - nb_from) * int(nv)
     return res
+
+
+def _sized(res: DeviceResult) -> DeviceResult:
+    res.n_cols = res.device_ptrs()["n_cols"]
+    return res
+
+
+def rank_decompress(ctx: Context, rs: "DeviceRS", res: DeviceResult, flags: int = 0, result: DeviceResult | None = None) -> DeviceResult:
+    """bmb200_rank_decompress (rank_compressor::decompress): every group of `res`, read as bits of the compressed index space
+    of the NOT-NULL vector `rs` was built on, mapped to its logical positions.  The result has n_groups * rs.dset.n_blocks
+    columns, group-major."""
+    out = result if result is not None else DeviceResult(ctx)
+    ctx.check(lib().bmb200_rank_decompress(ctx._h, rs._h, res._h, int(flags), C.byref(out._h)), "rank_decompress")
+    return _sized(out)
+
+
+def rank_compress(ctx: Context, rs: "DeviceRS", src_vec: int, flags: int = 0, result: DeviceResult | None = None) -> DeviceResult:
+    """bmb200_rank_compress (rank_compressor::compress): vector src_vec of the set `rs` was built on, restricted to the
+    NOT-NULL vector and packed to its ranks; one group of max(1, ceil(count / 65536)) columns."""
+    out = result if result is not None else DeviceResult(ctx)
+    ctx.check(lib().bmb200_rank_compress(ctx._h, rs._h, int(src_vec), int(flags), C.byref(out._h)), "rank_compress")
+    return _sized(out)
 
 
 def aggregate_host(ctx: Context, ps, op: int, group0, group1=None, flags: int = 0):

@@ -12,6 +12,7 @@
 #include "aux_kernels.cuh"
 #include "runlist_kernel.cuh"
 #include "scan_kernel.cuh"
+#include "rank_kernel.cuh"
 #include "shift_kernel.cuh"
 #include "binop_kernel.cuh"
 #include <algorithm>
@@ -59,8 +60,8 @@ struct bmb200_ctx {
     uint8_t* h_ring[kStageSlots] = {};      // pinned staging ring of bmb200_set_upload_vectors (grow-only)
     size_t h_ring_cap = 0;
     cudaEvent_t ring_ev[kStageSlots] = {};
-    void* d_pool[8] = {};                   // grow-only device scratch of the fetch / rank / select entry points (no cudaMalloc per call)
-    size_t d_pool_cap[8] = {};
+    void* d_pool[9] = {};                   // grow-only device scratch of the fetch / rank / select / rank-compress entry points (no cudaMalloc per call)
+    size_t d_pool_cap[9] = {};
     std::vector<std::pair<uint64_t, uint64_t>> mirror_sig;   // slab list (base, bytes) whose copies into d_pool[6] were queued last
     bool mirror_live = false;               // ... by bmb200_host_slabs_prefetch, not yet consumed by an upload
     void* h_pool[8] = {};                   // grow-only pinned scratch of the same entry points
@@ -2323,6 +2324,85 @@ int bmb200_rs_free(bmb200_rs* rs)
     cudaFree(rs->bcount); cudaFree(rs->sub_count); cudaFree(rs->row_cum); cudaFree(rs->sb_tot); cudaFree(rs->sb_cum);
     cudaFree(rs->fine); cudaFree(rs->fine_piv); cudaFree(rs->row_piv);
     delete rs;
+    return BMB200_OK;
+}
+
+/* ------------------------------------------------------------------ rank compression (rank_kernel.cuh) */
+
+// *inout recycled when it has the shape asked for, else freed and replaced (as bmb200_scan does)
+static int rank_result(bmb200_ctx* ctx, uint32_t n_cols, uint32_t n_groups, bool compress, bmb200_result** inout, bmb200_result** out)
+{
+    bmb200_result* r = *inout;
+    if (r && (r->ctx != ctx || r->n_cols != n_cols || r->n_groups != n_groups || !r->blocks || (compress && !r->gaps) || r->or_blocks)) {
+        bmb200_result_free(r); r = nullptr; *inout = nullptr;
+    }
+    if (!r) { int rc = result_alloc(ctx, n_cols, n_groups, true, compress, false, &r); if (rc) return rc; }
+    r->has_blocks = true; r->compress = compress; r->gaps_ready = compress;      // the epilogue writes the GAP form in compress mode
+    *out = r;
+    return BMB200_OK;
+}
+
+int bmb200_rank_decompress(bmb200_ctx* ctx, const bmb200_rs* idx, const bmb200_result* src, uint32_t flags, bmb200_result** inout)
+{
+    if (!ctx || !idx || !src || !inout || idx->ctx != ctx || src->ctx != ctx || *inout == src) return BMB200_ERR_BADARG;
+    if (flags & ~BMB200_F_OPT_COMPRESS) return BMB200_ERR_BADARG;
+    // the source's columns are read by their kind: BIT ones need the stored blocks, GAP ones the GAP form
+    if (!src->has_blocks || !src->blocks || !src->n_groups || src->n_cols != src->n_groups * src->cols_per_group ||
+        (src->compress && (!src->gaps || !src->gaps_ready))) return BMB200_ERR_BADARG;
+    const uint64_t tot_cols = (uint64_t)src->n_groups * idx->n_blocks;
+    if (tot_cols > 0x7fffffffull) return BMB200_ERR_RANGE;
+    CU(cudaSetDevice(ctx->device));
+    const bool compress = (flags & BMB200_F_OPT_COMPRESS) != 0;
+    bmb200_result* r = nullptr;
+    int rc = rank_result(ctx, (uint32_t)tot_cols, src->n_groups, compress, inout, &r);
+    if (rc) return rc;
+    auto bail = [&](int e) { if (!*inout) bmb200_result_free(r); return e; };
+    if (cudaMemsetAsync(r->total, 0, 8 * (size_t)r->n_groups, ctx->stream) != cudaSuccess) { ctx->last_err = "rank_decompress: memset"; return bail(BMB200_ERR_CUDA); }
+    AggParams p{};
+    p.n_groups = r->n_groups; p.n_cols = r->n_cols; p.compress = compress ? 1u : 0u; p.store_blocks = 1u;
+    p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
+    p.total = r->total;
+    RankSrc s{src->kind, src->blocks, src->gaps, src->cols_per_group};
+    uint32_t grid = (uint32_t)(ctx->sm_count * kCtasPerSm); if (grid > p.n_cols) grid = p.n_cols;
+    rank_decompress_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p, rs_view(idx), s);
+    if ((rc = after_launch(ctx))) return bail(rc);
+    *inout = r;
+    return BMB200_OK;
+}
+
+int bmb200_rank_compress(bmb200_ctx* ctx, const bmb200_rs* idx, uint32_t src_vec, uint32_t flags, bmb200_result** inout)
+{
+    if (!ctx || !idx || !inout || idx->ctx != ctx) return BMB200_ERR_BADARG;
+    if (flags & ~BMB200_F_OPT_COMPRESS) return BMB200_ERR_BADARG;
+    if (src_vec >= idx->set->v.n_vec) return BMB200_ERR_RANGE;
+    CU(cudaSetDevice(ctx->device));
+    uint64_t total = 0;                                   // count(NN) sizes the target
+    CU(cudaMemcpyAsync(&total, idx->sb_cum + idx->nsb, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    const uint64_t cols64 = total ? (total + 65535u) >> 16 : 1u;
+    if (cols64 > 0x7fffffffull) return BMB200_ERR_RANGE;
+    const uint32_t cols = (uint32_t)cols64;
+    const bool compress = (flags & BMB200_F_OPT_COMPRESS) != 0;
+    uint32_t* dense = nullptr;
+    int rc = pool_dev(ctx, 8, (size_t)cols * BMB200_BLOCK_BYTES, (void**)&dense);
+    if (rc) return rc;
+    bmb200_result* r = nullptr;
+    if ((rc = rank_result(ctx, cols, 1u, compress, inout, &r))) return rc;
+    auto bail = [&](int e) { if (!*inout) bmb200_result_free(r); return e; };
+    cudaError_t e = cudaMemsetAsync(dense, 0, (size_t)cols * BMB200_BLOCK_BYTES, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
+    if (e != cudaSuccess) { ctx->last_err = std::string("rank_compress: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
+    uint32_t grid = (uint32_t)(ctx->sm_count * kCtasPerSm); if (grid > idx->n_blocks) grid = idx->n_blocks;
+    rank_compress_scatter_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(rs_view(idx), src_vec, dense);
+    if ((rc = after_launch(ctx))) return bail(rc);
+    AggParams p{};
+    p.n_groups = 1; p.n_cols = cols; p.compress = compress ? 1u : 0u; p.store_blocks = 1u;
+    p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
+    p.total = r->total;
+    grid = (uint32_t)(ctx->sm_count * kCtasPerSm); if (grid > cols) grid = cols;
+    finalize_blocks_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p, dense);
+    if ((rc = after_launch(ctx))) return bail(rc);
+    *inout = r;
     return BMB200_OK;
 }
 

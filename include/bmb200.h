@@ -26,6 +26,9 @@
  *   bmb200_rs_build               <- bvector::build_rs_index       src/bm.h:2531-2660, rs_index src/bmrs.h:688-715
  *   bmb200_rank_batch             <- bvector::count_to             src/bm.h:3120-3167
  *   bmb200_select_batch           <- bvector::select               src/bm.h:5350-5385
+ *   bmb200_rank_decompress        <- rank_compressor::decompress   src/bmalgo.h:571-644,
+ *                                    sparse_vector_scanner::decompress src/bmsparsevec_algo.h:4525-4537
+ *   bmb200_rank_compress          <- rank_compressor::compress     src/bmalgo.h:498-566
  *
  * Block geometry (src/bmconst.h:55-68,78-87): a bit-block is 2048 x u32 =
  * 8192 B = 65536 bits; a GAP block is u16 buf[0..len], buf[0] = header
@@ -404,6 +407,25 @@ int bmb200_select_batch(bmb200_rs* rs, const uint64_t* rank, uint64_t n, uint64_
 int bmb200_rank_batch_dev(bmb200_rs* rs, const uint64_t* d_pos, uint64_t n, uint64_t* d_out);
 int bmb200_select_batch_dev(bmb200_rs* rs, const uint64_t* d_rank, uint64_t n, uint64_t* d_pos, uint8_t* d_found);
 int bmb200_rs_free(bmb200_rs* rs);
+
+/* ---------------- rank compression (rank-select compressed sparse vectors) ----------------
+ * A bm::rsc_sparse_vector<> (src/bmsparsevec_compr.h) keeps only its NOT-NULL elements in its bit-planes, packed to the
+ * positions [0, effective_size()); its NOT-NULL vector NN maps them back to the logical index space.  A search over it is a
+ * bmb200_scan over the compressed columns [0, ceil(effective_size / 65536)) with the universe [0, effective_size), followed
+ * by bmb200_rank_decompress with the rs index of NN (sparse_vector_scanner searches an RSC vector the same way,
+ * src/bmsparsevec_algo.h:2300-2306,4525-4537).  A count-only search needs no decompression: it is a bijection on the bits
+ * below count(NN), so the scan's group totals are already the answer.  flags: BMB200_F_OPT_NONE / BMB200_F_OPT_COMPRESS. */
+/* rank_compressor<BV>::decompress  src/bmalgo.h:571 ; sparse_vector_scanner::decompress src/bmsparsevec_algo.h:4525
+ * idx = the rs index of the NOT-NULL vector (bmb200_rs_build); src = any result whose columns start at compressed column 0
+ * (n_groups groups of cols_per_group columns).  Out: n_groups * n_blocks(idx) columns, group-major, like a pipeline batch.
+ * Bit p of group g is set iff NN[p] is set and bit rank_NN(p) - 1 of group g of src is set; compressed positions past the
+ * source's columns read as 0, positions >= count(NN) are never read. */
+int bmb200_rank_decompress(bmb200_ctx* ctx, const bmb200_rs* idx, const bmb200_result* src, uint32_t flags, bmb200_result** inout);
+/* rank_compressor<BV>::compress  src/bmalgo.h:498 ; src = vector src_vec of the set idx was built on; bits outside idx dropped.
+ * Out: one group of max(1, ceil(count(idx) / 65536)) columns.  Bit r is set iff src is set at the position of the (r+1)-th set
+ * bit of NN.  For src not a subset of NN the result is compress(src & NN); the reference requires src to be a subset
+ * (src/bmalgo.h:526-549, asserted only) and computes an unspecified result otherwise. */
+int bmb200_rank_compress(bmb200_ctx* ctx, const bmb200_rs* idx, uint32_t src_vec, uint32_t flags, bmb200_result** inout);
 
 #ifdef __cplusplus
 }
