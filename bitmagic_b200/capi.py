@@ -223,7 +223,7 @@ class Context:
         self.check(lib().bmb200_exchange_popcounts(res._h, int(cols_per_rank)), "exchange_popcounts")
 
     def exchange_mode(self) -> int:
-        """0 = no exchange yet, 1 = ncclAllGather on the side stream, 2 = peer-memory pushes (CUDA IPC over NVLink)"""
+        """0 = no exchange yet, 1 = ncclAllGather on the side stream"""
         m = C.c_int(0)
         self.check(lib().bmb200_exchange_mode(self._h, C.byref(m)), "exchange_mode")
         return m.value

@@ -23,11 +23,44 @@
 #include "blob_entropy.cuh"
 #include "host_pack.hpp"
 #include "comm.hpp"
-#include "xchg_kernel.cuh"
 #include <sched.h>
 #include <fstream>
 
 using namespace bmb200;
+
+// Slots of the context's grow-only scratch (pool_dev / pool_host), one per buffer and role.  Entry points that do the same job share
+// a slot: bmb200_result_fetch and bmb200_result_fetch_view compact through the same buffers, rank and select batches stage through
+// the same ones.
+enum DevSlot {
+    kDevCompactOff,                   // compaction of a result: per-column offsets
+    kDevCompactBits,                  //   compacted bit-blocks
+    kDevCompactGaps,                  //   compacted GAP words
+    kDevRsIn,                         // bmb200_rank_batch / bmb200_select_batch: positions or ranks in
+    kDevRsOut,                        //   ranks or positions out
+    kDevRsFound,                      //   select's found flags
+    kDevSlabMirror,                   // bmb200_set_upload_slabs: the device mirror of the slabs (freed by bmb200_ctx_trim)
+    kDevSlabSrc,                      //   where each block sits in the mirror (freed by bmb200_ctx_trim)
+    kDevRankDense,                    // bmb200_rank_compress: the dense scatter target
+    kDevBlobStage,                    // bmb200_set_upload_blobs: the BLOB bytes
+    kDevBlobOff, kDevBlobSize,        //   per-vector offset and size inside the staged bytes
+    kDevBlobToks, kDevBlobNToks,      //   pass 1: token table, tokens per segment
+    kDevBlobStatus, kDevBlobFull,     //   status words, FULL-block flags
+    kDevBlobScratch,                  //   per-warp decode scratch
+    kDevBlobSegs, kDevBlobSegCap,     //   pass 1: segments, their token capacities and processing order
+    kDevBlobRecs, kDevBlobERecs,      //   decode records: explicit-length tokens, entropy-coded tokens
+    kDevBlobDur,                      //   pass 2: clocks per work item (BMB200_TRACE)
+    kDevSlots
+};
+enum HostSlot {
+    kHostCompactOff,                  // bmb200_result_fetch: staging of the per-column offsets
+    kHostExchange,                    // bmb200_exchange_fetch: the gathered rows
+    kHostViewMeta,                    // bmb200_result_fetch_view: kind | nruns | totals | offsets
+    kHostViewBits0, kHostViewGaps0,   //   its two block buffers, used in turn (see there)
+    kHostViewBits1, kHostViewGaps1,
+    kHostSlabSrc,                     // bmb200_set_upload_slabs: staging of the block sources
+    kHostBlobStage,                   // bmb200_set_upload_blobs: the BLOB bytes, gathered for one DMA
+    kHostSlots
+};
 
 struct bmb200_ctx {
     int device = 0;
@@ -45,11 +78,6 @@ struct bmb200_ctx {
     int agg_ctas_per_sm = kCtasPerSm;
     bmb200_set* host_set = nullptr;         // device arena kept between bmb200_aggregate_host calls (cudaMalloc/cudaFree
     bmb200_result* host_res = nullptr;      //   of a multi-GB arena costs tens of ms per call otherwise)
-    size_t cap_desc = 0, cap_base = 0, cap_bit = 0, cap_gap = 0;
-    uint8_t* h_stage = nullptr;             // pinned staging for serialized BLOBs (bmb200_set_upload_blobs), grown on demand
-    size_t h_stage_cap = 0;
-    void* d_tmp[13] = {};                   // device temporaries of bmb200_set_upload_blobs (staging, token tables, decode scratch): kept
-    size_t d_tmp_cap[13] = {};              //   between calls, grown on demand -- cudaMalloc / cudaFree of a few hundred MB costs tens of ms each
     int gap_mode = 0;                       // 0 = stream sorted GAP lists through the smem ring, 1 = always gather
     bool attr_set = false, merge_attr_set = false;
     size_t agg_dyn[4] = {};                 // dynamic shared memory per agg_kernel<OP> (set_agg_attrs)
@@ -60,12 +88,12 @@ struct bmb200_ctx {
     uint8_t* h_ring[kStageSlots] = {};      // pinned staging ring of bmb200_set_upload_vectors (grow-only)
     size_t h_ring_cap = 0;
     cudaEvent_t ring_ev[kStageSlots] = {};
-    void* d_pool[9] = {};                   // grow-only device scratch of the fetch / rank / select / rank-compress entry points (no cudaMalloc per call)
-    size_t d_pool_cap[9] = {};
-    std::vector<std::pair<uint64_t, uint64_t>> mirror_sig;   // slab list (base, bytes) whose copies into d_pool[6] were queued last
+    void* d_pool[kDevSlots] = {};           // grow-only device scratch by DevSlot (no cudaMalloc per call once warm)
+    size_t d_pool_cap[kDevSlots] = {};
+    std::vector<std::pair<uint64_t, uint64_t>> mirror_sig;   // slab list (base, bytes) whose copies into kDevSlabMirror were queued last
     bool mirror_live = false;               // ... by bmb200_host_slabs_prefetch, not yet consumed by an upload
-    void* h_pool[8] = {};                   // grow-only pinned scratch of the same entry points
-    size_t h_pool_cap[8] = {};
+    void* h_pool[kHostSlots] = {};          // grow-only pinned scratch by HostSlot
+    size_t h_pool_cap[kHostSlots] = {};
     cudaEvent_t fetch_ev[8] = {};           // one per D2H chunk of bmb200_result_fetch_view_async
     unsigned fetch_flip = 0;                // bmb200_result_fetch_view alternates between two pinned block buffers (see there)
     CommState comm;                         // multi-GPU exchange (bmb200_comm_*), unused on one GPU
@@ -206,7 +234,7 @@ void free_result_arrays(bmb200_result* r)
 
 // grow-only scratch owned by the context: the hot entry points never call cudaMalloc / cudaMallocHost once warm.
 // The caller has synchronized (or is ordered on) the context stream before it reuses a slot.
-int pool_dev(bmb200_ctx* ctx, int slot, size_t bytes, void** out)
+int pool_dev(bmb200_ctx* ctx, DevSlot slot, size_t bytes, void** out)
 {
     if (bytes > ctx->d_pool_cap[slot]) {
         if (ctx->d_pool[slot]) { cudaStreamSynchronize(ctx->stream); cudaFree(ctx->d_pool[slot]); ctx->d_pool[slot] = nullptr; ctx->d_pool_cap[slot] = 0; }
@@ -218,7 +246,7 @@ int pool_dev(bmb200_ctx* ctx, int slot, size_t bytes, void** out)
     *out = ctx->d_pool[slot];
     return BMB200_OK;
 }
-int pool_host(bmb200_ctx* ctx, int slot, size_t bytes, void** out)
+int pool_host(bmb200_ctx* ctx, HostSlot slot, size_t bytes, void** out)
 {
     if (bytes > ctx->h_pool_cap[slot]) {
         if (ctx->h_pool[slot]) { cudaStreamSynchronize(ctx->stream); cudaFreeHost(ctx->h_pool[slot]); ctx->h_pool[slot] = nullptr; ctx->h_pool_cap[slot] = 0; }
@@ -231,77 +259,6 @@ int pool_host(bmb200_ctx* ctx, int slot, size_t bytes, void** out)
     return BMB200_OK;
 }
 
-// the peer-memory exchange buffer of this rank and its mappings of the other ranks' buffers.  Collective: every rank gets here at
-// the same exchange (or at comm_destroy); its own pushes are complete once its stream is synchronized, and the all-gather below is
-// the barrier after which nobody writes into a buffer that is about to be unmapped / freed.
-void xchg_release(bmb200_ctx* ctx)
-{
-    CommState& c = ctx->comm;
-    if (!c.xbuf) return;
-    cudaStreamSynchronize(ctx->stream);
-    if (c.comm && c.stage[0] && c.gathered[0]) {
-        nccl_api().AllGather(c.stage[0], c.gathered[0], 1, kNcclUint32, c.comm, c.side);
-        const auto t0 = std::chrono::steady_clock::now();               // a peer that is gone must not hang the teardown
-        while (cudaStreamQuery(c.side) == cudaErrorNotReady && std::chrono::steady_clock::now() - t0 < std::chrono::seconds(10))
-            std::this_thread::sleep_for(std::chrono::milliseconds(1));
-    }
-    for (int q = 0; q < c.nranks && q < 64; ++q) if (c.peer_map[q]) { cudaIpcCloseMemHandle(c.peer_map[q]); c.peer_map[q] = nullptr; }
-    cudaFree(c.xbuf); cudaFree(c.d_peers); cudaFree(c.d_err);
-    c.xbuf = nullptr; c.d_peers = nullptr; c.d_err = nullptr; c.direct = false; c.xwords = 0; c.xseq = 0;
-}
-
-// (re)build the peer-memory exchange for rows of `words` u32.  Collective.  On any failure on any rank every rank falls back to the
-// ncclAllGather path (c.direct stays false).
-void xchg_setup(bmb200_ctx* ctx, size_t words)
-{
-    CommState& c = ctx->comm;
-    xchg_release(ctx);
-    // ncclAllGather is the default and BMB200_EXCHANGE_DIRECT=1 selects the peer-memory pushes.
-    if (!getenv("BMB200_EXCHANGE_DIRECT") || c.nranks > 64 || c.nranks < 2) return;
-    struct Msg { cudaIpcMemHandle_t h; uint32_t ok; uint32_t pad[3]; };
-    static_assert(sizeof(Msg) % 4 == 0, "message in u32 words");
-    const size_t msg_words = sizeof(Msg) / 4;
-    if (msg_words > words) return;                                   // (the staging buffers carry the handles)
-    Msg mine; memset(&mine, 0, sizeof mine);
-    const size_t bytes = ((size_t)2 * c.nranks * words + (size_t)2 * c.nranks) * 4;
-    bool ok = cudaMalloc((void**)&c.xbuf, bytes) == cudaSuccess && cudaMemset(c.xbuf, 0, bytes) == cudaSuccess &&
-              cudaMalloc((void**)&c.d_peers, sizeof(uint32_t*) * (size_t)c.nranks) == cudaSuccess &&
-              cudaMalloc((void**)&c.d_err, 64) == cudaSuccess && cudaMemset(c.d_err, 0, 64) == cudaSuccess &&
-              cudaIpcGetMemHandle(&mine.h, c.xbuf) == cudaSuccess;
-    if (!ok) cudaGetLastError();
-    mine.ok = ok ? 1u : 0u;
-    std::vector<Msg> all((size_t)c.nranks);
-    auto gather = [&](const Msg& m) -> bool {                        // host-visible all-gather of one Msg per rank through the NCCL buffers
-        if (cudaMemcpy(c.stage[0], &m, sizeof m, cudaMemcpyHostToDevice) != cudaSuccess) return false;
-        if (nccl_api().AllGather(c.stage[0], c.gathered[0], msg_words, kNcclUint32, c.comm, c.side) != 0) return false;
-        if (cudaStreamSynchronize(c.side) != cudaSuccess) return false;
-        return cudaMemcpy(all.data(), c.gathered[0], sizeof(Msg) * (size_t)c.nranks, cudaMemcpyDeviceToHost) == cudaSuccess;
-    };
-    bool gathered = gather(mine);
-    std::vector<uint32_t*> peers((size_t)c.nranks, nullptr);
-    if (gathered) for (int q = 0; q < c.nranks; ++q) ok = ok && all[(size_t)q].ok;
-    if (gathered && ok) {
-        for (int q = 0; q < c.nranks && ok; ++q) {
-            if (q == c.rank) { peers[(size_t)q] = c.xbuf; continue; }
-            void* pmap = nullptr;
-            if (cudaIpcOpenMemHandle(&pmap, all[(size_t)q].h, cudaIpcMemLazyEnablePeerAccess) != cudaSuccess) { cudaGetLastError(); ok = false; break; }
-            c.peer_map[q] = pmap; peers[(size_t)q] = (uint32_t*)pmap;
-        }
-        if (ok) ok = cudaMemcpy(c.d_peers, peers.data(), sizeof(uint32_t*) * (size_t)c.nranks, cudaMemcpyHostToDevice) == cudaSuccess;
-    }
-    // second round: direct only if EVERY rank mapped every buffer
-    mine.ok = (gathered && ok) ? 1u : 0u;
-    bool all_ok = gather(mine);
-    if (all_ok) for (int q = 0; q < c.nranks; ++q) all_ok = all_ok && all[(size_t)q].ok;
-    if (!all_ok) { xchg_release(ctx); return; }
-    // both kernels run between two launches of the aggregation kernel, which needs the SMs' largest shared-memory carve-out: ask for
-    // the same split so that no SM has to be re-partitioned in between
-    cudaFuncSetAttribute(xchg_push_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    cudaFuncSetAttribute(xchg_wait_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-    c.direct = true; c.xwords = words; c.xseq = 0;
-}
-
 void comm_release(bmb200_ctx* ctx)
 {
     CommState& c = ctx->comm;
@@ -311,7 +268,6 @@ void comm_release(bmb200_ctx* ctx)
         if (c.done[k]) cudaEventDestroy(c.done[k]);
         cudaFree(c.stage[k]); cudaFree(c.gathered[k]);
     }
-    xchg_release(ctx);
     if (c.comm && nccl_api().CommDestroy) nccl_api().CommDestroy(c.comm);
     if (c.side) cudaStreamDestroy(c.side);
     c = CommState();
@@ -380,8 +336,6 @@ int bmb200_destroy(bmb200_ctx* ctx)
     if (ctx->own_stream) cudaStreamDestroy(ctx->stream);
     cudaFree(ctx->d_work); cudaFree(ctx->d_group);
     if (ctx->h_group) cudaFreeHost(ctx->h_group);
-    if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-    for (void* q : ctx->d_tmp) if (q) cudaFree(q);
     for (void* q : ctx->d_pool) if (q) cudaFree(q);
     for (void* q : ctx->h_pool) if (q) cudaFreeHost(q);
     for (uint32_t k = 0; k < kStageSlots; ++k) { if (ctx->h_ring[k]) cudaFreeHost(ctx->h_ring[k]); if (ctx->ring_ev[k]) cudaEventDestroy(ctx->ring_ev[k]); }
@@ -489,6 +443,22 @@ static int set_alloc(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, uint64_
     return BMB200_OK;
 }
 
+// H2D of one packed set into an arena from set_alloc that holds it (bmb200_set_upload, and bmb200_aggregate_host, which reuses its
+// arena across calls: the slack behind the GAP pool is zeroed again at the new end)
+static int set_copy_in(bmb200_ctx* ctx, bmb200_set* s, const bmb200_packed_set* h, uint64_t n_bit, uint64_t n_gap)
+{
+    cudaStream_t st = ctx->stream;
+    s->v.n_vec = h->n_vec; s->v.n_blocks = h->n_blocks; s->n_bit_blocks = n_bit; s->n_gap_units = n_gap;
+    s->gap_pool_bytes = n_gap * 16ull + kSlack;
+    CU(cudaMemcpyAsync((void*)s->v.desc, h->desc, (size_t)h->n_vec * h->n_blocks * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync((void*)s->v.bit_base, h->bit_base, ((size_t)h->n_blocks + 1) * 8, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync((void*)s->v.gap_base, h->gap_base, ((size_t)h->n_blocks + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (n_bit) CU(cudaMemcpyAsync((void*)s->v.bit_pool, h->bit_pool, (size_t)n_bit * BMB200_BLOCK_BYTES, cudaMemcpyHostToDevice, st));
+    if (n_gap) CU(cudaMemcpyAsync((void*)s->v.gap_pool, h->gap_pool, (size_t)n_gap * kGapUnit * 2, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync((char*)s->v.gap_pool + (size_t)n_gap * kGapUnit * 2, 0, kSlack, st));
+    return BMB200_OK;
+}
+
 int bmb200_set_upload(bmb200_ctx* ctx, const bmb200_packed_set* h, bmb200_set** out)
 {
     if (!ctx || !h || !out || !h->n_vec || !h->n_blocks || !h->desc || !h->bit_base || !h->gap_base)
@@ -499,20 +469,7 @@ int bmb200_set_upload(bmb200_ctx* ctx, const bmb200_packed_set* h, bmb200_set** 
     bmb200_set* s = nullptr;
     int rc = set_alloc(ctx, h->n_vec, h->n_blocks, n_bit, n_gap, &s);
     if (rc) return rc;
-    cudaStream_t st = ctx->stream;
-    cudaError_t e = cudaSuccess;
-    auto cp = [&](const void* dst, const void* src, size_t bytes) {
-        if (e == cudaSuccess && bytes) e = cudaMemcpyAsync((void*)dst, src, bytes, cudaMemcpyHostToDevice, st);
-    };
-    cp(s->v.desc, h->desc, (size_t)h->n_vec * h->n_blocks * 4);
-    cp(s->v.bit_base, h->bit_base, ((size_t)h->n_blocks + 1) * 8);
-    cp(s->v.gap_base, h->gap_base, ((size_t)h->n_blocks + 1) * 8);
-    cp(s->v.bit_pool, h->bit_pool, (size_t)n_bit * BMB200_BLOCK_BYTES);
-    cp(s->v.gap_pool, h->gap_pool, (size_t)n_gap * kGapUnit * 2);
-    if (e != cudaSuccess) {
-        ctx->last_err = std::string("set_upload memcpy: ") + cudaGetErrorString(e);
-        free_set_arrays(s); delete s; return BMB200_ERR_CUDA;
-    }
+    if ((rc = set_copy_in(ctx, s, h, n_bit, n_gap))) { free_set_arrays(s); delete s; return rc; }
     *out = s;
     return BMB200_OK;
 }
@@ -643,7 +600,7 @@ static int mirror_begin(bmb200_ctx* ctx, const bmb200_host_slab* slabs, uint32_t
     if (M.base.empty() || mirror_bytes > (128ull << 30)) return BMB200_OK;         // caller falls back to host packing
     CU(cudaSetDevice(ctx->device));
     uint8_t* mirror = nullptr;
-    int rc = pool_dev(ctx, 6, mirror_bytes + mirror_bytes / 16 + 64, (void**)&mirror);      // headroom: a heap that grew by a slab does not force a re-allocation
+    int rc = pool_dev(ctx, kDevSlabMirror, mirror_bytes + mirror_bytes / 16 + 64, (void**)&mirror);      // headroom: a heap that grew by a slab does not force a re-allocation
     if (rc) return rc;
     *mirror_out = mirror;
     if (ctx->mirror_live && ctx->mirror_sig == sig) { ctx->mirror_live = false; return BMB200_OK; }      // prefetched by bmb200_host_slabs_prefetch
@@ -689,7 +646,7 @@ int bmb200_set_upload_slabs(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, 
     bool inside = false;
     try {
         pack_layout(n_vec, n_blocks, vecs, (unsigned)ctx->host_threads, L);
-        if (!L.rc && !(rc = pool_host(ctx, 5, (size_t)n_vec * n_blocks * 4, (void**)&h_src)))
+        if (!L.rc && !(rc = pool_host(ctx, kHostSlabSrc, (size_t)n_vec * n_blocks * 4, (void**)&h_src)))
             inside = pack_sources(n_vec, n_blocks, vecs, L, M, (unsigned)ctx->host_threads, h_src);
     } catch (...) { rc = BMB200_ERR_BADALLOC; }
     if (L.rc || rc || !inside) {
@@ -702,7 +659,7 @@ int bmb200_set_upload_slabs(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, 
     bmb200_set* s = nullptr;
     if ((rc = set_alloc(ctx, n_vec, n_blocks, n_bit, n_gap, &s))) { cudaStreamSynchronize(st); return rc; }
     uint32_t* d_src = nullptr;
-    if ((rc = pool_dev(ctx, 7, (size_t)n_vec * n_blocks * 4, (void**)&d_src))) { cudaStreamSynchronize(st); free_set_arrays(s); delete s; return rc; }
+    if ((rc = pool_dev(ctx, kDevSlabSrc, (size_t)n_vec * n_blocks * 4, (void**)&d_src))) { cudaStreamSynchronize(st); free_set_arrays(s); delete s; return rc; }
     e = cudaMemcpyAsync(d_src, h_src, (size_t)n_vec * n_blocks * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync((void*)s->v.desc, L.desc.data(), L.desc.size() * 4, cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync((void*)s->v.bit_base, L.bb.data(), L.bb.size() * 8, cudaMemcpyHostToDevice, st);
@@ -840,41 +797,26 @@ int bmb200_set_upload_blobs(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, 
     // buffer so the copy is a single DMA at link speed instead of one pageable copy per vector
     uint8_t* d_stg = nullptr; BlobRec *d_recs = nullptr, *d_erecs = nullptr;
     uint64_t *d_boff = nullptr, *d_bsize = nullptr; BlobTok* d_toks = nullptr; uint32_t* d_ntoks = nullptr; int* d_status = nullptr;
-    uint8_t *d_full = nullptr, *d_scratch = nullptr;
+    uint8_t *d_full = nullptr, *d_scratch = nullptr, *h_stg = nullptr;
     bmb200_set* s = nullptr;
-    // temporaries live in the context's grow-only pool (slot i of ctx->d_tmp); the stream is synchronized before this function
-    // returns, so the next call may reuse them
-    auto tmp_alloc = [&](int slot, void** ptr, size_t bytes) -> cudaError_t {
-        if (bytes > ctx->d_tmp_cap[slot]) {
-            if (ctx->d_tmp[slot]) { cudaStreamSynchronize(st); cudaFree(ctx->d_tmp[slot]); ctx->d_tmp[slot] = nullptr; ctx->d_tmp_cap[slot] = 0; }
-            cudaError_t ae = cudaMalloc(&ctx->d_tmp[slot], bytes);
-            if (ae != cudaSuccess) return ae;
-            ctx->d_tmp_cap[slot] = bytes;
-        }
-        *ptr = ctx->d_tmp[slot];
-        return cudaSuccess;
-    };
+    // temporaries live in the context's grow-only pools (the kDevBlob* slots and kHostBlobStage); the stream is synchronized before
+    // this function returns, so the next call may reuse them
     auto fail = [&](int rc, cudaError_t e) {
         cudaStreamSynchronize(st);
-        if (rc == BMB200_ERR_CUDA || (!rc && e != cudaSuccess)) { ctx->last_err = std::string("set_upload_blobs: ") + cudaGetErrorString(e); rc = BMB200_ERR_CUDA; }
+        if (e != cudaSuccess && (!rc || rc == BMB200_ERR_CUDA)) { ctx->last_err = std::string("set_upload_blobs: ") + cudaGetErrorString(e); rc = BMB200_ERR_CUDA; }
         if (s) { free_set_arrays(s); delete s; }
         return rc;
     };
-    cudaError_t e = tmp_alloc(0, (void**)&d_stg, stg_bytes + 64);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_stg + stg_bytes, 0, 64, st);
-    if (e == cudaSuccess && stg_bytes > ctx->h_stage_cap) {
-        cudaStreamSynchronize(st);
-        if (ctx->h_stage) cudaFreeHost(ctx->h_stage);
-        ctx->h_stage = nullptr; ctx->h_stage_cap = 0;
-        e = cudaMallocHost((void**)&ctx->h_stage, stg_bytes);
-        if (e == cudaSuccess) ctx->h_stage_cap = stg_bytes;
-    }
+    int rc = pool_dev(ctx, kDevBlobStage, stg_bytes + 64, (void**)&d_stg);
+    if (!rc) rc = pool_host(ctx, kHostBlobStage, stg_bytes, (void**)&h_stg);
+    if (rc) return fail(rc, cudaSuccess);
+    cudaError_t e = cudaMemsetAsync(d_stg + stg_bytes, 0, 64, st);
     if (e == cudaSuccess) {
         cudaStreamSynchronize(st);                     // a previous call may still be reading the staging buffer
-        for (uint32_t v = 0; v < n_vec; ++v) memcpy(ctx->h_stage + stg_off[v], blobs[v].data, blobs[v].size);
-        e = cudaMemcpyAsync(d_stg, ctx->h_stage, stg_bytes, cudaMemcpyHostToDevice, st);
+        for (uint32_t v = 0; v < n_vec; ++v) memcpy(h_stg + stg_off[v], blobs[v].data, blobs[v].size);
+        e = cudaMemcpyAsync(d_stg, h_stg, stg_bytes, cudaMemcpyHostToDevice, st);
     }
-    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? BMB200_ERR_BADALLOC : BMB200_ERR_CUDA, e);
+    if (e != cudaSuccess) return fail(BMB200_ERR_CUDA, e);
     tr.mark("stage + H2D of BLOB bytes");
     const uint32_t ent_grid_max = (uint32_t)ctx->sm_count * 8u;       // warps that decode at the same time (one scratch slot each)
     uint32_t n_status = 0;                                             // d_status[n_status] = status word of pass 2
@@ -887,7 +829,7 @@ int bmb200_set_upload_blobs(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, 
         try {
             for (uint32_t v = 0; v < n_vec; ++v) {
                 const size_t first = segs.size();
-                int rc = ent_find_segments((const uint8_t*)blobs[v].data, blobs[v].size, v, stg_off[v], segs);
+                rc = ent_find_segments((const uint8_t*)blobs[v].data, blobs[v].size, v, stg_off[v], segs);
                 if (rc) return fail(rc, cudaSuccess);
                 for (size_t k = first; k < segs.size(); ++k) {            // token slots: one per block the segment can reach (+ super-block records)
                     const uint64_t lo = std::min<uint64_t>(segs[k].nb0, n_blocks);
@@ -900,16 +842,16 @@ int bmb200_set_upload_blobs(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, 
         } catch (...) { return fail(BMB200_ERR_BADALLOC, cudaSuccess); }
         const uint32_t n_segs = (uint32_t)segs.size();
         const uint32_t grid = std::min(n_segs, ent_grid_max);
-        if (e == cudaSuccess) e = tmp_alloc(1, (void**)&d_boff, 8ull * n_vec);
-        if (e == cudaSuccess) e = tmp_alloc(2, (void**)&d_bsize, 8ull * n_vec);
-        if (e == cudaSuccess) e = tmp_alloc(3, (void**)&d_toks, sizeof(BlobTok) * (size_t)tok_total);
-        if (e == cudaSuccess) e = tmp_alloc(4, (void**)&d_ntoks, 4ull * n_segs);
-        if (e == cudaSuccess) e = tmp_alloc(5, (void**)&d_status, 4ull * (n_segs + 3));
-        if (e == cudaSuccess) e = tmp_alloc(6, (void**)&d_full, (size_t)n_vec * n_blocks);
-        if (e == cudaSuccess) e = tmp_alloc(7, (void**)&d_scratch, (size_t)ent_grid_max * kEntScratchBytes);
-        if (e == cudaSuccess) e = tmp_alloc(10, (void**)&d_segs, sizeof(EntSeg) * (size_t)n_segs);
-        if (e == cudaSuccess) e = tmp_alloc(11, (void**)&d_segcap, 8ull * n_segs);            // capacities, then the processing order
-        if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? BMB200_ERR_BADALLOC : BMB200_ERR_CUDA, e);
+        if ((rc = pool_dev(ctx, kDevBlobOff, 8ull * n_vec, (void**)&d_boff)) ||
+            (rc = pool_dev(ctx, kDevBlobSize, 8ull * n_vec, (void**)&d_bsize)) ||
+            (rc = pool_dev(ctx, kDevBlobToks, sizeof(BlobTok) * (size_t)tok_total, (void**)&d_toks)) ||
+            (rc = pool_dev(ctx, kDevBlobNToks, 4ull * n_segs, (void**)&d_ntoks)) ||
+            (rc = pool_dev(ctx, kDevBlobStatus, 4ull * (n_segs + 3), (void**)&d_status)) ||
+            (rc = pool_dev(ctx, kDevBlobFull, (size_t)n_vec * n_blocks, (void**)&d_full)) ||
+            (rc = pool_dev(ctx, kDevBlobScratch, (size_t)ent_grid_max * kEntScratchBytes, (void**)&d_scratch)) ||
+            (rc = pool_dev(ctx, kDevBlobSegs, sizeof(EntSeg) * (size_t)n_segs, (void**)&d_segs)) ||
+            (rc = pool_dev(ctx, kDevBlobSegCap, 8ull * n_segs, (void**)&d_segcap)))           // capacities, then the processing order
+            return fail(rc, cudaSuccess);
         e = cudaMemcpyAsync(d_boff, stg_off.data(), 8ull * n_vec, cudaMemcpyHostToDevice, st);
         if (e == cudaSuccess) e = cudaMemcpyAsync(d_bsize, blob_size.data(), 8ull * n_vec, cudaMemcpyHostToDevice, st);
         if (e == cudaSuccess) e = cudaMemcpyAsync(d_segs, segs.data(), sizeof(EntSeg) * (size_t)n_segs, cudaMemcpyHostToDevice, st);
@@ -925,8 +867,7 @@ int bmb200_set_upload_blobs(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, 
         tr.mark("walk buffers");
         blob_walk_kernel<<<grid, kEntThreads, 0, st>>>(d_stg, d_segs, d_segcap, d_segcap + n_segs, (uint32_t*)d_status + n_segs + 1, n_segs, n_vec, n_blocks, d_toks,
                                                        d_ntoks, d_status, d_full, d_scratch);
-        int rc = after_launch(ctx);
-        if (rc) return fail(rc, cudaGetLastError());
+        if ((rc = after_launch(ctx))) return fail(rc, cudaGetLastError());
         tr.mark("blob_walk_kernel");
         std::vector<uint32_t> ntoks; std::vector<int> status; std::vector<BlobTok> all;
         try { ntoks.resize(n_segs); status.resize(n_segs); all.resize(tok_total); } catch (...) { return fail(BMB200_ERR_BADALLOC, cudaSuccess); }
@@ -994,11 +935,11 @@ int bmb200_set_upload_blobs(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, 
     const uint64_t n_bit = bb[n_blocks], n_gap = gb[n_blocks];
     std::stable_sort(erecs.begin(), erecs.end(), [](const BlobRec& a, const BlobRec& b) { return (a.aux2 >> 2) > (b.aux2 >> 2); });
     tr.mark("arena layout (host)");
-    int rc = set_alloc(ctx, n_vec, n_blocks, n_bit, n_gap, &s);
+    rc = set_alloc(ctx, n_vec, n_blocks, n_bit, n_gap, &s);
     if (rc) { s = nullptr; return fail(rc, cudaSuccess); }
-    if (!recs.empty()) e = tmp_alloc(8, (void**)&d_recs, recs.size() * sizeof(BlobRec));
-    if (e == cudaSuccess && !erecs.empty()) e = tmp_alloc(9, (void**)&d_erecs, erecs.size() * sizeof(BlobRec));
-    if (e != cudaSuccess) return fail(e == cudaErrorMemoryAllocation ? BMB200_ERR_BADALLOC : BMB200_ERR_CUDA, e);
+    if ((!recs.empty() && (rc = pool_dev(ctx, kDevBlobRecs, recs.size() * sizeof(BlobRec), (void**)&d_recs))) ||
+        (!erecs.empty() && (rc = pool_dev(ctx, kDevBlobERecs, erecs.size() * sizeof(BlobRec), (void**)&d_erecs))))
+        return fail(rc, cudaSuccess);
     if (!recs.empty()) e = cudaMemcpyAsync(d_recs, recs.data(), recs.size() * sizeof(BlobRec), cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess && !erecs.empty()) e = cudaMemcpyAsync(d_erecs, erecs.data(), erecs.size() * sizeof(BlobRec), cudaMemcpyHostToDevice, st);
     if (e == cudaSuccess) e = cudaMemcpyAsync((void*)s->v.desc, desc.data(), desc.size() * 4, cudaMemcpyHostToDevice, st);
@@ -1019,7 +960,7 @@ int bmb200_set_upload_blobs(bmb200_ctx* ctx, uint32_t n_vec, uint32_t n_blocks, 
         uint32_t grid = (uint32_t)std::min<size_t>(erecs.size(), (size_t)ent_grid_max);
         SetView sv{n_vec, n_blocks, s->v.desc, s->v.bit_base, s->v.gap_base, s->v.bit_pool, s->v.gap_pool};
         unsigned long long* d_dur = nullptr;
-        if (tr.on) { e = tmp_alloc(12, (void**)&d_dur, 8ull * erecs.size()); if (e != cudaSuccess) return fail(BMB200_ERR_CUDA, e); }
+        if (tr.on && (rc = pool_dev(ctx, kDevBlobDur, 8ull * erecs.size(), (void**)&d_dur))) return fail(rc, cudaSuccess);
         blob_entropy_kernel<<<grid, kEntThreads, 0, st>>>(d_stg, d_boff, d_bsize, d_erecs, (uint32_t)erecs.size(), (uint32_t*)d_status + n_status + 2, sv, (uint32_t*)s->v.bit_pool,
                                                           (uint16_t*)s->v.gap_pool, d_status + n_status, d_scratch, d_dur);
         if ((rc = after_launch(ctx))) return fail(rc, cudaGetLastError());
@@ -1156,7 +1097,7 @@ int bmb200_ctx_trim(bmb200_ctx* ctx)
     cudaStreamSynchronize(ctx->stream);
     auto& a = ctx->arena;
     if (a.full) { cudaFree(a.desc); cudaFree(a.bb); cudaFree(a.gb); cudaFree(a.bp); cudaFree(a.gp); a = bmb200_ctx::Arena(); }
-    for (int slot = 6; slot <= 7; ++slot)           // the slab mirror and its source table (bmb200_set_upload_slabs)
+    for (DevSlot slot : {kDevSlabMirror, kDevSlabSrc})
         if (ctx->d_pool[slot]) { cudaFree(ctx->d_pool[slot]); ctx->d_pool[slot] = nullptr; ctx->d_pool_cap[slot] = 0; }
     return BMB200_OK;
 }
@@ -1521,13 +1462,7 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     p.or_blocks = or_target ? r->or_blocks : nullptr;
     set_agg_attrs(ctx, &ce);
     if (ce != cudaSuccess) { ctx->last_err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(ce); return bail(BMB200_ERR_CUDA); }
-    uint32_t sms = (uint32_t)ctx->sm_count;
-    if (ctx->comm.comm && ctx->comm.nranks > 1 && ctx->sm_count > 8) {
-        // sharded runs: the all-gather of the previous step has to find SMs while this (persistent, SM-filling) kernel runs, or it
-        // waits for the gap between two aggregation kernels and stretches it; BMB200_AGG_RESERVE_SMS leaves that many SMs free
-        static const int reserve = []() { const char* e = getenv("BMB200_AGG_RESERVE_SMS"); return e ? atoi(e) : 0; }();
-        if (reserve > 0 && reserve < ctx->sm_count) sms = (uint32_t)(ctx->sm_count - reserve);
-    }
+    const uint32_t sms = (uint32_t)ctx->sm_count;
     uint32_t grid = sms * (uint32_t)ctx->agg_ctas_per_sm;
     if (grid > n_cols) grid = n_cols;
     RunLists rl{};
@@ -1805,8 +1740,10 @@ int bmb200_result_fetch(bmb200_result* r, uint8_t* kind_out, uint64_t* off_out, 
     if (!nb && !ng) return BMB200_OK;
     // compaction scratch and the offsets' staging come from the context's grow-only pools (no allocation once warm)
     uint64_t* d_off = nullptr; uint32_t* d_bits = nullptr; uint16_t* d_gaps = nullptr; uint64_t* h_off = nullptr;
-    if ((rc = pool_dev(ctx, 0, (size_t)r->n_cols * 8, (void**)&d_off)) || (rc = pool_dev(ctx, 1, (size_t)nb * BMB200_BLOCK_BYTES + 16, (void**)&d_bits)) ||
-        (rc = pool_dev(ctx, 2, (size_t)ng * 2 + 16, (void**)&d_gaps)) || (rc = pool_host(ctx, 0, (size_t)r->n_cols * 8, (void**)&h_off))) return rc;
+    if ((rc = pool_dev(ctx, kDevCompactOff, (size_t)r->n_cols * 8, (void**)&d_off)) ||
+        (rc = pool_dev(ctx, kDevCompactBits, (size_t)nb * BMB200_BLOCK_BYTES + 16, (void**)&d_bits)) ||
+        (rc = pool_dev(ctx, kDevCompactGaps, (size_t)ng * 2 + 16, (void**)&d_gaps)) ||
+        (rc = pool_host(ctx, kHostCompactOff, (size_t)r->n_cols * 8, (void**)&h_off))) return rc;
     memcpy(h_off, off.data(), (size_t)r->n_cols * 8);
     CU(cudaMemcpyAsync(d_off, h_off, (size_t)r->n_cols * 8, cudaMemcpyHostToDevice, ctx->stream));
     uint32_t grid = (uint32_t)ctx->sm_count * 8u; if (grid > r->n_cols) grid = r->n_cols;
@@ -1828,7 +1765,7 @@ static int fetch_view_impl(bmb200_result* r, const uint8_t** kind_out, const uin
     // one pinned block of the context: kind | nruns | totals | off ; two stream synchronisations per call, no allocation once warm
     const size_t n = r->n_cols, o_nr = (n + 7) & ~(size_t)7, o_tot = o_nr + n * 4 + ((n & 1) ? 4 : 0), o_off = o_tot + 8 * (size_t)r->n_groups;
     uint8_t* h = nullptr;
-    int rc = pool_host(ctx, 2, o_off + n * 8, (void**)&h);
+    int rc = pool_host(ctx, kHostViewMeta, o_off + n * 8, (void**)&h);
     if (rc) return rc;
     uint8_t* kind = h; uint32_t* nruns = (uint32_t*)(h + o_nr); uint64_t* tot = (uint64_t*)(h + o_tot); uint64_t* off = (uint64_t*)(h + o_off);
     CU(cudaMemcpyAsync(kind, r->kind, n, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1848,14 +1785,15 @@ static int fetch_view_impl(bmb200_result* r, const uint8_t** kind_out, const uin
     uint32_t* hb = nullptr; uint16_t* hg = nullptr;
     if (nb || ng) {
         uint64_t* d_off = nullptr; uint32_t* d_bits = nullptr; uint16_t* d_gaps = nullptr;
-        if ((rc = pool_dev(ctx, 0, n * 8, (void**)&d_off)) || (rc = pool_dev(ctx, 1, (size_t)nb * BMB200_BLOCK_BYTES + 16, (void**)&d_bits)) ||
-            (rc = pool_dev(ctx, 2, (size_t)ng * 2 + 16, (void**)&d_gaps)) ||
-            false) return rc;
+        if ((rc = pool_dev(ctx, kDevCompactOff, n * 8, (void**)&d_off)) ||
+            (rc = pool_dev(ctx, kDevCompactBits, (size_t)nb * BMB200_BLOCK_BYTES + 16, (void**)&d_bits)) ||
+            (rc = pool_dev(ctx, kDevCompactGaps, (size_t)ng * 2 + 16, (void**)&d_gaps))) return rc;
         // two pinned buffers, used in turn: the caller's threads have just READ the previous call's blocks, which parks those lines in
         // their private L2 caches, and a DMA write into lines cached by many cores has to snoop every one of them, which makes
         // it several times slower than a write into cold lines)
-        const int fb = (ctx->fetch_flip ^= 1u) ? 6 : 3, fg = fb + 1;
-        if ((rc = pool_host(ctx, fb, (size_t)nb * BMB200_BLOCK_BYTES + 16, (void**)&hb)) || (rc = pool_host(ctx, fg, (size_t)ng * 2 + 16, (void**)&hg))) return rc;
+        const bool flip = (ctx->fetch_flip ^= 1u) != 0;
+        if ((rc = pool_host(ctx, flip ? kHostViewBits1 : kHostViewBits0, (size_t)nb * BMB200_BLOCK_BYTES + 16, (void**)&hb)) ||
+            (rc = pool_host(ctx, flip ? kHostViewGaps1 : kHostViewGaps0, (size_t)ng * 2 + 16, (void**)&hg))) return rc;
         CU(cudaMemcpyAsync(d_off, off, n * 8, cudaMemcpyHostToDevice, ctx->stream));
         uint32_t grid = (uint32_t)ctx->sm_count * 8u; if (grid > r->n_cols) grid = r->n_cols;
         result_compact_kernel<<<grid, 256, 0, ctx->stream>>>(r->blocks, r->gaps, r->kind, d_off, d_bits, d_gaps, r->n_cols);
@@ -1937,21 +1875,6 @@ int bmb200_result_free(bmb200_result* r)
     return BMB200_OK;
 }
 
-// H2D of one packed set into an existing device arena (capacities checked by the caller)
-static int set_copy_in(bmb200_ctx* ctx, bmb200_set* s, const bmb200_packed_set* h, uint64_t n_bit, uint64_t n_gap)
-{
-    cudaStream_t st = ctx->stream;
-    s->v.n_vec = h->n_vec; s->v.n_blocks = h->n_blocks; s->n_bit_blocks = n_bit; s->n_gap_units = n_gap;
-    s->gap_pool_bytes = n_gap * 16ull + kSlack;
-    CU(cudaMemcpyAsync((void*)s->v.desc, h->desc, (size_t)h->n_vec * h->n_blocks * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync((void*)s->v.bit_base, h->bit_base, ((size_t)h->n_blocks + 1) * 8, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync((void*)s->v.gap_base, h->gap_base, ((size_t)h->n_blocks + 1) * 8, cudaMemcpyHostToDevice, st));
-    if (n_bit) CU(cudaMemcpyAsync((void*)s->v.bit_pool, h->bit_pool, (size_t)n_bit * BMB200_BLOCK_BYTES, cudaMemcpyHostToDevice, st));
-    if (n_gap) CU(cudaMemcpyAsync((void*)s->v.gap_pool, h->gap_pool, (size_t)n_gap * kGapUnit * 2, cudaMemcpyHostToDevice, st));
-    CU(cudaMemsetAsync((char*)s->v.gap_pool + (size_t)n_gap * kGapUnit * 2, 0, kSlack, st));
-    return BMB200_OK;
-}
-
 int bmb200_aggregate_host(bmb200_ctx* ctx, const bmb200_packed_set* host, const bmb200_agg_args* args,
                           const bmb200_result_meta* meta_out, uint64_t* total_out)
 {
@@ -1962,11 +1885,11 @@ int bmb200_aggregate_host(bmb200_ctx* ctx, const bmb200_packed_set* host, const 
     if ((n_bit && !host->bit_pool) || (n_gap && !host->gap_pool)) return BMB200_ERR_BADARG;
     const size_t need_desc = (size_t)host->n_vec * host->n_blocks, need_base = (size_t)host->n_blocks + 1;
     // the device arena and the result buffers persist in the context: every call still copies ALL inputs H2D
-    if (!ctx->host_set || need_desc > ctx->cap_desc || need_base > ctx->cap_base || n_bit > ctx->cap_bit || n_gap > ctx->cap_gap) {
+    const bmb200_set* hs = ctx->host_set;
+    if (!hs || need_desc > hs->cap_desc || need_base > hs->cap_base || n_bit > hs->cap_bit || n_gap > hs->cap_gap) {
         if (ctx->host_set) { bmb200_set_free(ctx->host_set); ctx->host_set = nullptr; }
         int rc = set_alloc(ctx, host->n_vec, host->n_blocks, n_bit, n_gap, &ctx->host_set);
         if (rc) return rc;
-        ctx->cap_desc = need_desc; ctx->cap_base = need_base; ctx->cap_bit = n_bit; ctx->cap_gap = n_gap;
     }
     int rc = set_copy_in(ctx, ctx->host_set, host, n_bit, n_gap);
     if (!rc) rc = bmb200_aggregate(ctx, ctx->host_set, args, &ctx->host_res);
@@ -2052,28 +1975,13 @@ int bmb200_exchange_popcounts(bmb200_result* r, uint32_t cols_per_rank)
             CU(cudaMalloc((void**)&c.gathered[k], words * 4 * (size_t)c.nranks));
         }
         c.cap_cols = n;
-        xchg_setup(ctx, words);
-    }
-    if (c.direct) {
-        // the library's own exchange: this rank's row goes into every peer's buffer by peer stores, right behind the aggregation kernel
-        XchgParams xp{};
-        xp.peers = c.d_peers; xp.nranks = (uint32_t)c.nranks; xp.rank = (uint32_t)c.rank; xp.xwords = (uint32_t)c.xwords;
-        xp.seq = (uint32_t)(++c.xseq); xp.slot = xp.seq & 1u;
-        xp.n_cols = r->n_cols; xp.n = (uint32_t)n; xp.popcnt = r->popcnt; xp.total = r->total; xp.err = c.d_err;
-        xp.timeout_ns = 30ull * 1000000000ull;
-        xchg_push_kernel<<<(unsigned)c.nranks, 256, 0, ctx->stream>>>(xp);
-        int rcl = after_launch(ctx);
-        if (rcl) return rcl;
-        c.cols[xp.slot] = (uint32_t)n; c.seq++;
-        return BMB200_OK;
     }
     const int k = (int)(c.seq % (uint64_t)CommState::kSlots);
     // slot k was last used by the exchange kSlots steps back: nothing below may overtake that all-gather
     if (c.pending[k]) CU(cudaStreamWaitEvent(ctx->stream, c.done[k], 0));
-    static const bool no_direct = getenv("BMB200_EXCHANGE_STAGED") != nullptr;
     const uint32_t* send = c.stage[k];
-    if (r->total_inline && n == r->n_cols && !(n & 1u) && !no_direct)
-        send = r->popcnt;                                       // (popcnt | total) as the kernel wrote them: no staging copy
+    if (r->total_inline && n == r->n_cols && !(n & 1u))
+        send = r->popcnt;                                      // (popcnt | total) as the kernel wrote them: no staging copy
     else {
         if (n > r->n_cols) CU(cudaMemsetAsync(c.stage[k] + r->n_cols, 0, (n - r->n_cols) * 4, ctx->stream));     // ragged shards: zero padding
         CU(cudaMemcpyAsync(c.stage[k], r->popcnt, (size_t)r->n_cols * 4, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -2092,7 +2000,7 @@ int bmb200_exchange_popcounts(bmb200_result* r, uint32_t cols_per_rank)
 int bmb200_exchange_mode(const bmb200_ctx* ctx, int* mode)
 {
     if (!ctx || !mode) return BMB200_ERR_BADARG;
-    *mode = (!ctx->comm.comm || !ctx->comm.seq) ? 0 : (ctx->comm.direct ? 2 : 1);
+    *mode = (!ctx->comm.comm || !ctx->comm.seq) ? 0 : 1;
     return BMB200_OK;
 }
 
@@ -2101,11 +2009,6 @@ int bmb200_exchange_fence(bmb200_ctx* ctx)
     if (!ctx || !ctx->comm.comm) return BMB200_ERR_BADARG;
     CU(cudaSetDevice(ctx->device));
     CommState& c = ctx->comm;
-    if (c.direct) {
-        if (!c.xseq) return BMB200_OK;
-        xchg_wait_kernel<<<1, 64, 0, ctx->stream>>>(c.xbuf, (uint32_t)c.nranks, (uint32_t)c.xwords, (uint32_t)(c.xseq & 1u), (uint32_t)c.xseq, c.d_err, 30ull * 1000000000ull);
-        return after_launch(ctx);
-    }
     for (int k = 0; k < CommState::kSlots; ++k) if (c.pending[k]) CU(cudaStreamWaitEvent(ctx->stream, c.done[k], 0));
     return BMB200_OK;
 }
@@ -2115,36 +2018,15 @@ int bmb200_exchange_fetch(bmb200_ctx* ctx, uint64_t* global_total, uint64_t* ran
     if (!ctx || !ctx->comm.comm || !ctx->comm.seq) return BMB200_ERR_BADARG;
     CommState& c = ctx->comm;
     CU(cudaSetDevice(ctx->device));
-    int k = (int)((c.seq - 1) % (uint64_t)CommState::kSlots);
-    const uint32_t* rows = nullptr;
-    size_t words = 0, n = 0;
-    if (c.direct) {
-        if (!c.xseq) return BMB200_ERR_BADARG;
-        k = (int)(c.xseq & 1u);
-        n = c.cols[k]; words = c.xwords;
-        int rcw = bmb200_exchange_fence(ctx);
-        if (rcw) return rcw;
-        uint32_t err = 0;
-        CU(cudaMemcpyAsync(&err, c.d_err, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (err) { ctx->last_err = "exchange: a peer did not publish its row within 30 s"; return BMB200_ERR_CUDA; }
-        if (getenv("BMB200_TRACE")) {
-            unsigned long long st[4] = {0, 0, 0, 0};
-            cudaMemcpy(st, c.d_err + 2, sizeof st, cudaMemcpyDeviceToHost);
-            fprintf(stderr, "[bmb200] exchange (peer memory), last push: flow-control wait %.1f us, row stores + fence %.1f us, flag %.1f us\n",
-                    (st[1] - st[0]) / 1e3, (st[2] - st[1]) / 1e3, (st[3] - st[2]) / 1e3);
-        }
-        rows = c.xbuf + (size_t)k * c.nranks * c.xwords;
-    } else {
-        n = c.cols[k]; words = n + 2;
-        CU(cudaEventSynchronize(c.done[k]));
-        rows = c.gathered[k];
-    }
+    const int k = (int)((c.seq - 1) % (uint64_t)CommState::kSlots);
+    const size_t n = c.cols[k], words = n + 2;
+    CU(cudaEventSynchronize(c.done[k]));
+    const uint32_t* rows = c.gathered[k];
     if (d_gathered) *d_gathered = rows;
     if (stride) *stride = (uint32_t)words;
     if (global_total || rank_totals || popcnt) {
         uint32_t* h = nullptr;
-        int rc = pool_host(ctx, 1, words * 4 * (size_t)c.nranks, (void**)&h);
+        int rc = pool_host(ctx, kHostExchange, words * 4 * (size_t)c.nranks, (void**)&h);
         if (rc) return rc;
         CU(cudaMemcpyAsync(h, rows, words * 4 * (size_t)c.nranks, cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
@@ -2290,7 +2172,7 @@ int bmb200_rank_batch(bmb200_rs* rs, const uint64_t* pos, uint64_t n, uint64_t* 
     CU(cudaSetDevice(ctx->device));
     uint64_t *d_in = nullptr, *d_out = nullptr;       // context pools: no cudaMalloc / cudaFree per call
     int rc;
-    if ((rc = pool_dev(ctx, 3, n * 8, (void**)&d_in)) || (rc = pool_dev(ctx, 4, n * 8, (void**)&d_out))) return rc;
+    if ((rc = pool_dev(ctx, kDevRsIn, n * 8, (void**)&d_in)) || (rc = pool_dev(ctx, kDevRsOut, n * 8, (void**)&d_out))) return rc;
     CU(cudaMemcpyAsync(d_in, pos, n * 8, cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = bmb200_rank_batch_dev(rs, d_in, n, d_out))) return rc;
     CU(cudaMemcpyAsync(out, d_out, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2307,7 +2189,8 @@ int bmb200_select_batch(bmb200_rs* rs, const uint64_t* rank, uint64_t n, uint64_
     CU(cudaSetDevice(ctx->device));
     uint64_t *d_in = nullptr, *d_pos = nullptr; uint8_t* d_f = nullptr;
     int rc;
-    if ((rc = pool_dev(ctx, 3, n * 8, (void**)&d_in)) || (rc = pool_dev(ctx, 4, n * 8, (void**)&d_pos)) || (rc = pool_dev(ctx, 5, n, (void**)&d_f))) return rc;
+    if ((rc = pool_dev(ctx, kDevRsIn, n * 8, (void**)&d_in)) || (rc = pool_dev(ctx, kDevRsOut, n * 8, (void**)&d_pos)) ||
+        (rc = pool_dev(ctx, kDevRsFound, n, (void**)&d_f))) return rc;
     CU(cudaMemcpyAsync(d_in, rank, n * 8, cudaMemcpyHostToDevice, ctx->stream));
     if ((rc = bmb200_select_batch_dev(rs, d_in, n, d_pos, d_f))) return rc;
     CU(cudaMemcpyAsync(pos, d_pos, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -2384,7 +2267,7 @@ int bmb200_rank_compress(bmb200_ctx* ctx, const bmb200_rs* idx, uint32_t src_vec
     const uint32_t cols = (uint32_t)cols64;
     const bool compress = (flags & BMB200_F_OPT_COMPRESS) != 0;
     uint32_t* dense = nullptr;
-    int rc = pool_dev(ctx, 8, (size_t)cols * BMB200_BLOCK_BYTES, (void**)&dense);
+    int rc = pool_dev(ctx, kDevRankDense, (size_t)cols * BMB200_BLOCK_BYTES, (void**)&dense);
     if (rc) return rc;
     bmb200_result* r = nullptr;
     if ((rc = rank_result(ctx, cols, 1u, compress, inout, &r))) return rc;

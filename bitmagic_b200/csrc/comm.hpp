@@ -66,14 +66,6 @@ struct CommState {
     uint32_t cols[kSlots] = {};               // columns of the exchange in flight in each slot
     uint64_t seq = 0;                        // exchanges issued
     bool pending[kSlots] = {};
-    // direct exchange over peer memory (xchg_kernel.cuh): the default when every rank could map every other rank's buffer
-    bool direct = false;
-    uint32_t* xbuf = nullptr;                // [2][nranks][xwords] rows + [2][nranks] flags; cudaMalloc, exported through CUDA IPC
-    uint32_t** d_peers = nullptr;            // device array [nranks]
-    void* peer_map[64] = {};                 // what cudaIpcOpenMemHandle returned for each peer (closed on release)
-    size_t xwords = 0;
-    uint32_t* d_err = nullptr;               // set by a wait that timed out (a peer died): the next fetch reports BMB200_ERR_CUDA
-    uint64_t xseq = 0;                       // exchanges pushed into the current xbuf
     const uint32_t* sendbuf[kSlots] = {};   // what the all-gather of each slot reads (a staging buffer or the result's own popcount buffer)
 };
 

@@ -12,9 +12,6 @@
 #include <cstdint>
 #include <cstdlib>
 #include <cstring>
-#if defined(__SSE2__)
-#include <emmintrin.h>
-#endif
 #include <mutex>
 #include <sched.h>
 #include <thread>
@@ -139,34 +136,13 @@ inline bool pack_sources(uint32_t n_vec, uint32_t n_blocks, const bmb200_vec_blo
     return true;
 }
 
-// 8 KB block -> staging slot with non-temporal stores (BMB200_PACK_NT=1): the slot is written once and then read by the DMA engine
-// only, so the read-for-ownership of a cached store and the later write-back are pure memory-bandwidth overhead next to the DMA.
-// Both pointers are 16-byte aligned (blocks: BM_ALLOC_ALIGN >= 16; slot offsets are multiples of 8 KB / 16 B).
-inline bool pack_nt_enabled() { static const bool on = getenv("BMB200_PACK_NT") != nullptr; return on; }
-inline void copy_block_nt(void* dst, const void* src)
-{
-#if defined(__SSE2__)
-    if (!(((uintptr_t)dst | (uintptr_t)src) & 15u)) {
-        const __m128i* s = (const __m128i*)src; __m128i* d = (__m128i*)dst;
-        for (unsigned i = 0; i < BMB200_BLOCK_BYTES / 16u; i += 4) {
-            const __m128i a = _mm_load_si128(s + i), b = _mm_load_si128(s + i + 1), c = _mm_load_si128(s + i + 2), e = _mm_load_si128(s + i + 3);
-            _mm_stream_si128(d + i, a); _mm_stream_si128(d + i + 1, b); _mm_stream_si128(d + i + 2, c); _mm_stream_si128(d + i + 3, e);
-        }
-        return;
-    }
-#endif
-    memcpy(dst, src, BMB200_BLOCK_BYTES);
-}
-
 // one column into its place inside a staging slot: bit-blocks at bit_dst (in descriptor order), GAP units at gap_dst
 inline void pack_column(uint32_t n_vec, uint32_t nb, const bmb200_vec_blocks* vecs, const uint32_t* drow, uint8_t* bit_dst, uint8_t* gap_dst)
 {
-    const bool nt = pack_nt_enabled();
     for (uint32_t v = 0; v < n_vec; ++v) {
         const uint32_t d = drow[v], kd = d & 3u;
         if (kd == BMB200_BLK_BIT) {
-            uint8_t* dst = bit_dst + (size_t)((d >> 2) & BMB200_DESC_REL_MASK) * BMB200_BLOCK_BYTES;
-            if (nt) copy_block_nt(dst, vecs[v].ptr[nb]); else memcpy(dst, vecs[v].ptr[nb], BMB200_BLOCK_BYTES);
+            memcpy(bit_dst + (size_t)((d >> 2) & BMB200_DESC_REL_MASK) * BMB200_BLOCK_BYTES, vecs[v].ptr[nb], BMB200_BLOCK_BYTES);
         } else if (kd == BMB200_BLK_GAP) {
             const uint16_t* g = (const uint16_t*)vecs[v].ptr[nb];
             const uint32_t words = (uint32_t)(g[0] >> 3) + 1u, pad = d >> 31;
@@ -177,9 +153,6 @@ inline void pack_column(uint32_t n_vec, uint32_t nb, const bmb200_vec_blocks* ve
             for (uint32_t i = n; i < npad; ++i) dst[i] = 0;             // FLAT contract: zeros up to the next unit (slots are recycled)
         }
     }
-#if defined(__SSE2__)
-    if (nt) _mm_sfence();        // non-temporal stores are weakly ordered: they must be globally visible before the chunk is reported complete
-#endif
 }
 
 // column chunks sized for one staging slot
@@ -274,8 +247,7 @@ struct PackPipeline {
         uint32_t before;
         { std::lock_guard<std::mutex> lk(mu); before = released; released = c; }
         // chunks [before + kStageSlots, c + kStageSlots) became admissible: wake the slots they live in (at most all of them)
-        static const bool herd = getenv("BMB200_PACK_WAKE_ALL") != nullptr;          // A/B switch: wake every slot's waiters on every release
-        const uint32_t span = (herd || c - before >= kStageSlots) ? kStageSlots : c - before;
+        const uint32_t span = c - before >= kStageSlots ? kStageSlots : c - before;
         for (uint32_t k = 0; k < span; ++k) cv_free[(before + k) % kStageSlots].notify_all();
     }
     void join()

@@ -671,7 +671,7 @@ public:
         if (to_ > from_) ds_.assign(vecs, n, from_, to_); else ds_.release();
         agg_.set_device_set(&ds_);
     }
-    /// transport of the exchange: 2 = peer-memory pushes over NVLink (CUDA IPC), 1 = ncclAllGather, 0 = nothing exchanged yet
+    /// transport of the exchange: 1 = ncclAllGather, 0 = nothing exchanged yet
     int exchange_mode() const { int m = 0; bmb200_exchange_mode(ctx_.get(), &m); return m; }
     uint32_t shard_from() const { return from_; }
     uint32_t shard_to() const { return to_; }

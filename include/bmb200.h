@@ -372,15 +372,11 @@ int bmb200_comm_info(const bmb200_ctx* ctx, int* nranks, int* rank);
 int bmb200_comm_destroy(bmb200_ctx* ctx);
 /* exchange of the local result `res` (single group) with all ranks; asynchronous, ordered after the work already queued on the
  * context stream; buffered three deep (the aggregation of step i never waits for the exchange of step i-1 or i-2).  Collective: every rank issues the same
- * sequence of exchanges.  Two transports (bmb200_exchange_mode):
- *   1 = one ncclAllGather of the rows on the context's SIDE stream (the default: the faster of the two where it was measured);
- *   2 = peer memory (BMB200_EXCHANGE_DIRECT=1): every rank's exchange buffer is mapped by every other rank through CUDA IPC and
- *       a small kernel behind the aggregation kernel stores this rank's (popcounts | cardinality) row into all of them over
- *       NVLink and publishes a sequence number; falls back to 1 when a rank cannot map a peer.
+ * sequence of exchanges.  The transport is one ncclAllGather of the rows on the context's SIDE stream.
  * cols_per_rank = the width of the widest shard (the same value on every rank; narrower shards are zero-padded), 0 = the
  * result's own column count when all shards are equal. */
 int bmb200_exchange_popcounts(bmb200_result* res, uint32_t cols_per_rank);
-/* *mode = 0 before the first exchange (or without a communicator), else the transport in use (see above) */
+/* *mode = 0 before the first exchange (or without a communicator), else 1 (ncclAllGather) */
 int bmb200_exchange_mode(const bmb200_ctx* ctx, int* mode);
 /* make the context stream wait for every exchange issued so far (asynchronous) */
 int bmb200_exchange_fence(bmb200_ctx* ctx);

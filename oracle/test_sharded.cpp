@@ -78,7 +78,7 @@ int main(int argc, char** argv)
         bvect shard_ref(t_ref); shard_ref &= mask;
         CHECK(shard_ref.compare(t_gpu) == 0, "pass %d: rank %d target != reference restricted to blocks [%u, %u)", pass, rank, from, to);
     }
-    std::printf("%s: rank %d/%d blocks [%u, %u): %d checks, %d failed; exchange mode %d (2 = peer memory, 1 = ncclAllGather)\n",
+    std::printf("%s: rank %d/%d blocks [%u, %u): %d checks, %d failed; exchange mode %d (1 = ncclAllGather)\n",
                 g_fail ? "FAILED" : "OK", rank, nranks, from, to, g_checks, g_fail, sh.exchange_mode());
     return g_fail ? 1 : 0;
 }
