@@ -1005,23 +1005,27 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
 // holds no listed bit-block either.
 // Protocol (no wait can outlive the producer): the producer claims a column only when a queue slot is free, publishes (item, #bit
 // stages, GAP bytes, first stage) and then issues all of the column's stages in order, each after its empty barrier; after the last
-// column it publishes an end marker.  Consumers read every queue entry, wait for exactly the stages the entry announces and release
-// each of them exactly once (bit stage: every warp arrives; GAP stage: its one reader arrives for all 16).  They free the queue slot
-// once the column is classified, because classification reads the column's listed flags that the producer staged with the entry.
-// With part B the entry's bit stages are the column's unlisted bit-blocks in order; stage j is the j-th of them.
-// Parity waits are only sound when the waiter has seen the stage's previous fill complete.  Bit stages (streamed ones only, with
-// part B) are still waited for by every warp in order; GAP or companion stage g still goes to warp g % 16, so with a ring of a
-// multiple of 16 stages the previous fill of each stage a warp waits for was one of its own GAP stages, or a bit stage / an earlier
-// column that every warp has finished.
+// column it publishes an end marker.  Consumers read every queue entry and wait for exactly the stages it announces: every warp
+// waits for every bit stage (one 16-byte word per thread); GAP or companion stage g of the column goes to the kPipeGroup warps of
+// group g % kPipeGroups, each sweeping its kPipeSlice bytes of it.  Every waiter arrives once on the stage's empty barrier, for
+// 16 / (its waiters) warps, so a stage is free as soon as its slowest slice is done and the rest of the ring stays requested.
+// They free the queue slot once the column is classified, because classification reads the column's listed flags that the
+// producer staged with the entry.  With part B the entry's bit stages are the column's unlisted bit-blocks in order.
+// Parity waits are sound because every waiter has waited for every earlier fill of the stage: fills of earlier columns all
+// completed before the column barriers the waiter has passed, and within a column a ring slot is reused only by bit stages,
+// which every warp waits for, or by GAP stages of the same warp group (kPipeStages is a multiple of kPipeGroups).
 constexpr int      kPipeStages  = 16;                      // 128 KB of stages
 constexpr uint32_t kPipeStage   = 8192u;
+constexpr uint32_t kPipeGroup   = 2u;                      // consumer warps that share one GAP or companion stage (DESIGN §3.1a: 1, 4, 8, 16 were slower)
+constexpr uint32_t kPipeGroups  = kAggWarps / kPipeGroup;  // GAP stage g of a column goes to warp group g % kPipeGroups
+constexpr uint32_t kPipeSlice   = kPipeStage / kPipeGroup; // bytes of such a stage each warp of its group sweeps
 constexpr int      kPipeQueue   = 2;                       // columns claimed ahead of the consumers (more would unbalance the tail)
 constexpr uint32_t kPipeMaxVec  = 4096u;                   // role table size: larger sets take agg_kernel
 constexpr int      kPipePerThr  = (int)kPipeMaxVec / kAggThreads;
 constexpr uint32_t kPipeMaxAndGap = 64u;                   // AND-group GAP blocks per column the FLAT path takes (more: in-place reads)
 constexpr uint32_t kPipeThreads = kAggThreads + 32u;       // 16 consumer warps + 1 producer warp
 constexpr size_t   kPipeRingSmem = (size_t)kPipeStages * kPipeStage;
-static_assert(kPipeStages % kAggWarps == 0, "GAP stage g is consumed by warp g % 16: the ring must hold a multiple of 16 stages");
+static_assert(kPipeStages % kPipeGroups == 0, "a ring slot must go to the same warp group each time a column reuses it");
 
 // *bad |= 1 when a GAP block of the set is not in the BMB200_DESC_GAP_FLAT form (agg_pipe_kernel sweeps SUB-group blocks as FLAT pairs)
 __global__ void desc_flat_check_kernel(const uint32_t* __restrict__ desc, size_t n, uint32_t* bad)
@@ -1233,22 +1237,25 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
         }
         agg_sync<true>();
 
-        // ---- GAP phase: GAP stage g belongs to warp g % 16 ----
+        // ---- GAP phase: GAP stage g goes to warp group g % kPipeGroups; a warp sweeps bytes [wlo, wlo + kPipeSlice) of it ----
         const uint32_t ngs = (gbytes + kPipeStage - 1u) / kPipeStage;
+        const uint32_t grp = (uint32_t)warp / kPipeGroup, wlo = ((uint32_t)warp % kPipeGroup) * kPipeSlice;
         if (rl.sgl_base) {
             // run-list companion: every GAP block is a SUB-group block, so the phase clears the column's singles (stages 0 .. ngs-1)
             // and long runs (the stages behind them) from L; no lead-pad repair, no AND-group blocks
             const uint32_t nst = ngs + (lbytes + kPipeStage - 1u) / kPipeStage;
             uint32_t flat_mode = 0;
-            for (uint32_t g = (uint32_t)warp; g < nst; g += kAggWarps) {
+            for (uint32_t g = grp; g < nst; g += kPipeGroups) {
                 const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
-                const uint32_t src = ring_s + s * kPipeStage + (uint32_t)lane * 16u;
+                const bool sgl = g < ngs;
+                const uint32_t bytes = sgl ? min(kPipeStage, gbytes - g * kPipeStage) : min(kPipeStage, lbytes - (g - ngs) * kPipeStage);
+                const uint32_t src = ring_s + s * kPipeStage + wlo + (uint32_t)lane * 16u, sb = bytes > wlo ? bytes - wlo : 0u;
                 mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
                 flat_update_mode(flat_mode, Ks, (uint32_t)lane, g);
-                if (g < ngs) sgl_sweep_fn(Ks, src, min(kPipeStage, gbytes - g * kPipeStage), (uint32_t)lane * 16u, flat_mode);
-                else         flat_sweep_fn(Ks, src, min(kPipeStage, lbytes - (g - ngs) * kPipeStage), (uint32_t)lane * 16u, flat_mode);
+                if (sgl) sgl_sweep_fn(Ks, src, min(kPipeSlice, sb), (uint32_t)lane * 16u, flat_mode);      // a partial last stage
+                else     flat_sweep_fn(Ks, src, min(kPipeSlice, sb), (uint32_t)lane * 16u, flat_mode);     // leaves later slices empty
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&s_empty[s], kAggWarps);
+                if (lane == 0) mbar_arrive(&s_empty[s], kPipeGroups);
             }
         } else if (flat) {
             // a FLAT SUB-group block without lead pad starts with a 1-run whose pair slot holds the header: clear that whole run here
@@ -1263,14 +1270,15 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
                 gap_scatter_gather<false>(Ks, gseg + (size_t)((d >> 2) & kRelMask) * kGapUnit + (d >> 31), 0u, lane);
             }
             uint32_t flat_mode = 0;
-            for (uint32_t g = (uint32_t)warp; g < ngs; g += kAggWarps) {
+            for (uint32_t g = grp; g < ngs; g += kPipeGroups) {
                 const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
+                const uint32_t st0 = g * kPipeStage, bytes = min(kPipeStage, gbytes - st0), sb = bytes > wlo ? bytes - wlo : 0u;
                 mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
-                if (nag) {   // blank the staged bytes of AND-group blocks: as zero pairs the sweep reads no run in them
-                    const uint32_t st0 = g * kPipeStage, st1 = st0 + min(kPipeStage, gbytes - st0);
+                if (nag) {   // blank the AND-group bytes of this warp's slice: as zero pairs the sweep reads no run in them
+                    const uint32_t w0 = st0 + wlo, w1 = w0 + min(kPipeSlice, sb);
                     for (uint32_t i = 0; i < nag; ++i) {
                         const uint2 a = s_ag[b][i];
-                        const uint32_t bs = max(((a.x >> 2) & kRelMask) * 16u, st0), be = min(a.y, st1);
+                        const uint32_t bs = max(((a.x >> 2) & kRelMask) * 16u, w0), be = min(a.y, w1);
                         for (uint32_t x = bs + 2u * (uint32_t)lane; x < be; x += 64u)
                             asm volatile("st.shared.u16 [%0], %1;" :: "r"(ring_s + s * kPipeStage + (x - st0)), "h"((uint16_t)0) : "memory");
                     }
@@ -1278,15 +1286,15 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
                     __syncwarp();
                 }
                 flat_update_mode(flat_mode, Ks, (uint32_t)lane, g);
-                flat_sweep_fn(Ks, ring_s + s * kPipeStage + (uint32_t)lane * 16u, min(kPipeStage, gbytes - g * kPipeStage), (uint32_t)lane * 16u, flat_mode);
+                flat_sweep_fn(Ks, ring_s + s * kPipeStage + wlo + (uint32_t)lane * 16u, min(kPipeSlice, sb), (uint32_t)lane * 16u, flat_mode);
                 __syncwarp();
-                if (lane == 0) mbar_arrive(&s_empty[s], kAggWarps);
+                if (lane == 0) mbar_arrive(&s_empty[s], kPipeGroups);
             }
         } else {
-            for (uint32_t g = (uint32_t)warp; g < ngs; g += kAggWarps) {      // release the staged segment unread
+            for (uint32_t g = 0; g < ngs; ++g) {                      // release the staged segment unread
                 const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
                 mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
-                if (lane == 0) mbar_arrive(&s_empty[s], kAggWarps);
+                if (lane == 0) mbar_arrive(&s_empty[s]);
             }
 #pragma unroll
             for (int i = 0; i < kPipePerThr; ++i) {            // this warp's 32 vectors of trip i, one GAP block at a time
