@@ -129,6 +129,7 @@ struct bmb200_result {
     uint32_t n_cols = 0;                    // total columns = n_groups * cols_per_group
     uint32_t n_groups = 1, cols_per_group = 0;
     uint32_t* or_blocks = nullptr;          // [cols_per_group][2048] union of all groups (BMB200_F_OR_TARGET)
+    bool has_or = false;                    // the last launch into this result filled or_blocks (a recycled result keeps the buffer)
     bool has_blocks = false, compress = false, gaps_ready = false;
     uint32_t* blocks = nullptr;
     uint32_t* popcnt = nullptr;
@@ -1440,7 +1441,7 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
         if (rc) return rc;
     }
     auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
-    r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
+    r->has_blocks = store; r->compress = compress; r->gaps_ready = false; r->has_or = or_target;
     if (r->total_inline && ctx->comm.comm) {
         r->xflip = (r->xflip + 1u) % (uint32_t)CommState::kSlots;
         r->popcnt = r->popcnt_base + (size_t)r->xflip * r->xstride;
@@ -1614,7 +1615,7 @@ int bmb200_result_group_totals(bmb200_result* r, uint64_t* totals, uint32_t n_gr
 
 int bmb200_result_or_target(bmb200_result* r, bmb200_result** out)
 {
-    if (!r || !out || !r->or_blocks) return BMB200_ERR_BADARG;
+    if (!r || !out || !r->or_blocks || !r->has_or) return BMB200_ERR_BADARG;
     bmb200_ctx* ctx = r->ctx;
     CU(cudaSetDevice(ctx->device));
     bmb200_result* o = nullptr;

@@ -289,7 +289,9 @@ int bmb200_binop(bmb200_ctx* ctx, const bmb200_set* set, int op, uint32_t va, ui
 int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_batch_args* args, bmb200_result** inout);
 /* per-group cardinalities (pipeline::get_bv_count_vector) */
 int bmb200_result_group_totals(bmb200_result* res, uint64_t* totals, uint32_t n_groups);
-/* finalize the OR target of a batch launched with BMB200_F_OR_TARGET into its own n_cols-column result */
+/* finalize the OR target of a batch launched with BMB200_F_OR_TARGET into its own n_cols-column result.  Only the LAST launch
+ * into res counts: BMB200_ERR_BADARG when it was made without BMB200_F_OR_TARGET (also when res was recycled from a call
+ * that had one), so a stale union is never returned */
 int bmb200_result_or_target(bmb200_result* res, bmb200_result** out);
 /* classify every result column like opt_copy_bit_block and convert runs < 1276 to GAP on device */
 int bmb200_result_optimize(bmb200_result* res);

@@ -240,24 +240,43 @@ int ref_aggregate_horizontal(const bmb200_packed_set* s, const bmb200_agg_args* 
     } catch (...) { return 1; }
 }
 
-/* bvector 3-operand ops (src/bm.h:1745-1850): target.bit_and(a,b,opt) etc.; op: 0 OR 1 AND 2 SUB 3 XOR */
+/* bvector 3-operand ops (src/bm.h:1745-1850): t.bit_and(a,b,opt) etc.; op: 0 OR 1 AND 2 SUB 3 XOR; false for any other op */
+static bool run_binop(const bmb200_packed_set* s, int op, uint32_t va, uint32_t vb, int compress, bvect& t)
+{
+    bvect a, b;
+    build_bvector(s, va, 0, s->n_blocks, a);
+    build_bvector(s, vb, 0, s->n_blocks, b);
+    bvect::optmode om = compress ? bvect::opt_compress : bvect::opt_none;
+    switch (op) {
+    case 0: t.bit_or(a, b, om); return true;
+    case 1: t.bit_and(a, b, om); return true;
+    case 2: t.bit_sub(a, b, om); return true;
+    case 3: t.bit_xor(a, b, om); return true;
+    default: return false;
+    }
+}
+
 int ref_binop(const bmb200_packed_set* s, int op, uint32_t va, uint32_t vb, int compress,
               uint8_t* kind, uint32_t* popcnt, uint32_t* blocks, uint64_t* count_out)
 {
     try {
-        bvect a, b, t;
-        build_bvector(s, va, 0, s->n_blocks, a);
-        build_bvector(s, vb, 0, s->n_blocks, b);
-        bvect::optmode om = compress ? bvect::opt_compress : bvect::opt_none;
-        switch (op) {
-        case 0: t.bit_or(a, b, om); break;
-        case 1: t.bit_and(a, b, om); break;
-        case 2: t.bit_sub(a, b, om); break;
-        case 3: t.bit_xor(a, b, om); break;
-        default: return 2;
-        }
+        bvect t;
+        if (!run_binop(s, op, va, vb, compress, t)) return 2;
         if (count_out) *count_out = t.count();
         export_bvector(t, s->n_blocks, kind, popcnt, blocks, 0);
+        return 0;
+    } catch (...) { return 1; }
+}
+
+/* ref_binop with the GAP words of the result as well (header with its capacity level + run ends, zero-filled past the
+ * block), so that the block kinds and GAP levels the two-operand ops store can be compared word for word */
+int ref_binop_gaps(const bmb200_packed_set* s, int op, uint32_t va, uint32_t vb, int compress,
+                   uint8_t* kind, uint32_t* popcnt, uint32_t* blocks, uint16_t* gaps)
+{
+    try {
+        bvect t;
+        if (!run_binop(s, op, va, vb, compress, t)) return 2;
+        export_bvector(t, s->n_blocks, kind, popcnt, blocks, gaps);
         return 0;
     } catch (...) { return 1; }
 }
