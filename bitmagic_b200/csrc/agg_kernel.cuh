@@ -156,12 +156,12 @@ __device__ __forceinline__ void mbar_arrive(uint64_t* bar, uint32_t count = 1u)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" :: "r"(smem_u32(bar)), "r"(count) : "memory");
 }
-// Block barrier over the kAggThreads threads that compute a column: the whole CTA (__syncthreads) in agg_kernel, named barrier 1
+// Block barrier over the NT threads that compute a column: the whole CTA (__syncthreads) in agg_kernel, named barrier 1
 // over the consumer warps in agg_pipe_kernel (PIPE), whose producer warp never joins it.
-template <bool PIPE>
+template <bool PIPE, int NT = kAggThreads>
 __device__ __forceinline__ void agg_sync()
 {
-    if (PIPE) asm volatile("bar.sync 1, %0;" :: "n"(kAggThreads) : "memory");
+    if (PIPE) asm volatile("bar.sync 1, %0;" :: "n"(NT) : "memory");
     else      __syncthreads();
 }
 
@@ -466,45 +466,63 @@ __host__ __device__ __forceinline__ uint32_t binop_rule(uint32_t op, uint32_t ka
     }
 }
 
-// Epilogue shared by agg_kernel, agg_pipe_kernel and finalize_blocks_kernel: R = this thread's 4 words of the result block.
-// state: 0 = nothing stored, 1 = FULL, 2 = computed block.  Fuses bit_block_count, calc_block_digest0,
+// Epilogue shared by agg_kernel, agg_pipe_kernel and finalize_blocks_kernel: R = this thread's WPT words of the result block, held by
+// NT = 2048 / WPT threads as WPT / 4 quarters of uint4: R[h] = words [4 (h NT + tid), 4 (h NT + tid) + 4) -- one uint4 per thread for
+// the 512-thread kernels, two for the 256 consumer threads of agg_pipe_kernel (so every LDS.128 / store of a quarter is conflict-free
+// and coalesced).  state: 0 = nothing stored, 1 = FULL, 2 = computed block.  Fuses bit_block_count, calc_block_digest0,
 // bit_block_calc_change, the opt_copy_bit_block classification and its bit_to_gap branch
 // (src/bmfunc.h:5808,1239,6040,5540; src/bmblocks.h:1355-1409).
-template <bool EMPTY_DIGEST_IS_NULL, bool PIPE = false>
-__device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, uint32_t colx, uint32_t grp, uint4 R, int state,
-                                             uint32_t* K, uint32_t* s_pc, uint32_t* s_tr, uint32_t* s_dg, uint32_t rule = 0u)
+template <int N> struct Quads { uint4 q[N]; };     // a thread's words of a result block (finish_block)
+template <bool EMPTY_DIGEST_IS_NULL, bool PIPE = false, int WPT = 4>
+__device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, uint32_t colx, uint32_t grp, const Quads<WPT / 4> Rv,
+                                             int state, uint32_t* K, uint32_t* s_pc, uint32_t* s_tr, uint32_t* s_dg, uint32_t rule = 0u)
 {
+    static_assert(WPT == 4 || WPT == 8, "a thread holds one or two uint4 of the result block");
+    constexpr int H = WPT / 4, NT = (int)kBlockWords / WPT, NW = NT / 32;
+    const uint4 (&R)[H] = Rv.q;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint4* K4 = reinterpret_cast<uint4*>(K);
-    // popcount, digest (4 waves per warp: 8 threads x 4 words = one 32-word wave), run ends
-    K4[tid] = R;                 // reuse K so each thread can see its right neighbour's first word
-    const uint32_t nz = (R.x | R.y | R.z | R.w) != 0u;
-    const uint32_t bal = __ballot_sync(0xffffffffu, nz);
-    uint32_t dg4 = 0;
+    // popcount, digest (4 waves per warp and quarter: 8 threads x 4 words = one 32-word wave), run ends
+    uint32_t dg4 = 0, pc = 0;    // dg4 bit 4h + q = wave q of this warp's quarter h is not empty
 #pragma unroll
-    for (int q = 0; q < 4; ++q) if ((bal >> (8 * q)) & 0xffu) dg4 |= (1u << q);
-    uint32_t pc = warp_sum(popc4(R));
-    agg_sync<PIPE>();
+    for (int h = 0; h < H; ++h) {
+        K4[h * NT + tid] = R[h];     // reuse K so each thread can see its right neighbour's first word
+        const uint32_t nz = (R[h].x | R[h].y | R[h].z | R[h].w) != 0u;
+        const uint32_t bal = __ballot_sync(0xffffffffu, nz);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) if ((bal >> (8 * q)) & 0xffu) dg4 |= (1u << (4 * h + q));
+        pc += popc4(R[h]);
+    }
+    pc = warp_sum(pc);
+    agg_sync<PIPE, NT>();
     // x has a bit at every position p whose successor differs (bit_block_calc_change src/bmfunc.h:6040 counts
     // them; bit_block_to_gap src/bmfunc.h:5540 emits them as run ends); bit 65535 has no successor
-    const uint32_t nxt = (tid + 1 < kAggThreads) ? (K[4 * tid + 4] & 1u) : (R.w >> 31);
-    const uint32_t x0 = R.x ^ ((R.x >> 1) | (R.y << 31)), x1 = R.y ^ ((R.y >> 1) | (R.z << 31));
-    const uint32_t x2 = R.z ^ ((R.z >> 1) | (R.w << 31)), x3 = R.w ^ ((R.w >> 1) | (nxt << 31));
-    const uint32_t cnt = __popc(x0) + __popc(x1) + __popc(x2) + __popc(x3);
-    uint32_t inc = cnt;          // inclusive warp scan of the run-end counts
+    uint32_t x[H][4], cnt[H];
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+        const uint4 r = R[h];
+        const uint32_t nxt = (h < H - 1 || tid + 1 < NT) ? (K[4 * (h * NT + tid) + 4] & 1u) : (r.w >> 31);
+        x[h][0] = r.x ^ ((r.x >> 1) | (r.y << 31)); x[h][1] = r.y ^ ((r.y >> 1) | (r.z << 31));
+        x[h][2] = r.z ^ ((r.z >> 1) | (r.w << 31)); x[h][3] = r.w ^ ((r.w >> 1) | (nxt << 31));
+        cnt[h] = __popc(x[h][0]) + __popc(x[h][1]) + __popc(x[h][2]) + __popc(x[h][3]);
+    }
+    // inclusive warp scan of the run-end counts; with two quarters both are scanned at once, quarter 1 in the high 16 bits
+    // (a quarter has at most 32768 run ends, so the low field never carries)
+    uint32_t inc = H == 1 ? cnt[0] : cnt[0] | (cnt[H - 1] << 16);
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
     if (lane == 31) s_tr[warp] = inc;
     if (lane == 0) { s_pc[warp] = pc; s_dg[warp] = dg4; }
-    agg_sync<PIPE>();
+    agg_sync<PIPE, NT>();
     uint32_t tpc = 0, ttr = 0, woff = 0; uint64_t dg = 0;
 #pragma unroll
-    for (int w = 0; w < kAggWarps; ++w) {
+    for (int w = 0; w < NW; ++w) {
         const uint32_t t = s_tr[w];
         tpc += s_pc[w]; ttr += t; if (w < warp) woff += t;
-        dg |= (uint64_t)s_dg[w] << (4 * w);
+        if (H == 1) dg |= (uint64_t)s_dg[w] << (4 * w);
+        else        dg |= ((uint64_t)(s_dg[w] & 0xfu) << (4 * w)) | ((uint64_t)(s_dg[w] >> 4) << (4 * NW + 4 * w));
     }
-    const uint32_t runs = ttr + 1u;
+    const uint32_t runs = H == 1 ? ttr + 1u : (ttr & 0xffffu) + (ttr >> 16) + 1u;
 
     // result kind: aggregator stores nothing when the AND/SUB/XOR digest is empty; otherwise
     // copy_bit_block (opt_none) or the opt_copy_bit_block classification (src/bmblocks.h:1355-1409)
@@ -530,28 +548,39 @@ __device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, u
     else kd = BMB200_BLK_BIT;
 
     if (p.or_blocks && kd != BMB200_BLK_NULL) {      // pipeline OR target: union of all group results of this column
-        uint32_t* ob = p.or_blocks + (size_t)colx * kBlockWords + 4u * tid;
-        if (R.x) atomicOr(ob + 0, R.x);
-        if (R.y) atomicOr(ob + 1, R.y);
-        if (R.z) atomicOr(ob + 2, R.z);
-        if (R.w) atomicOr(ob + 3, R.w);
+#pragma unroll
+        for (int h = 0; h < H; ++h) {
+            uint32_t* ob = p.or_blocks + (size_t)colx * kBlockWords + 4u * (h * NT + tid);
+            if (R[h].x) atomicOr(ob + 0, R[h].x);
+            if (R[h].y) atomicOr(ob + 1, R[h].y);
+            if (R[h].z) atomicOr(ob + 2, R[h].z);
+            if (R[h].w) atomicOr(ob + 3, R[h].w);
+        }
     }
-    if (p.store_blocks && kd == BMB200_BLK_BIT)
-        st_stream_v4(reinterpret_cast<uint4*>(p.blocks) + (size_t)col * (kBlockWords / 4) + tid, R);
+    if (p.store_blocks && kd == BMB200_BLK_BIT) {
+#pragma unroll
+        for (int h = 0; h < H; ++h)
+            st_stream_v4(reinterpret_cast<uint4*>(p.blocks) + (size_t)col * (kBlockWords / 4) + h * NT + tid, R[h]);
+    }
     if (p.store_blocks && kd == BMB200_BLK_GAP) {
         // bit -> GAP fused here (the bit_to_gap branch of opt_copy_bit_block): run ends in order, header last
         uint16_t* gout = p.gaps + (size_t)col * kGapMax;
-        uint32_t off = 1u + woff + inc - cnt;
-        const uint32_t base = 128u * tid;
-        uint32_t m;
-        m = x0; while (m) { const uint32_t b = __ffs(m) - 1u; m &= m - 1u; gout[off++] = (uint16_t)(base + b); }
-        m = x1; while (m) { const uint32_t b = __ffs(m) - 1u; m &= m - 1u; gout[off++] = (uint16_t)(base + 32u + b); }
-        m = x2; while (m) { const uint32_t b = __ffs(m) - 1u; m &= m - 1u; gout[off++] = (uint16_t)(base + 64u + b); }
-        m = x3; while (m) { const uint32_t b = __ffs(m) - 1u; m &= m - 1u; gout[off++] = (uint16_t)(base + 96u + b); }
+#pragma unroll
+        for (int h = 0; h < H; ++h) {
+            uint32_t off = H == 1 ? 1u + woff + inc - cnt[0]
+                         : h == 0 ? 1u + (woff & 0xffffu) + (inc & 0xffffu) - cnt[0]
+                                  : 1u + (ttr & 0xffffu) + (woff >> 16) + (inc >> 16) - cnt[h];
+            const uint32_t base = 128u * (h * NT + tid);
+            uint32_t m;
+            m = x[h][0]; while (m) { const uint32_t b = __ffs(m) - 1u; m &= m - 1u; gout[off++] = (uint16_t)(base + b); }
+            m = x[h][1]; while (m) { const uint32_t b = __ffs(m) - 1u; m &= m - 1u; gout[off++] = (uint16_t)(base + 32u + b); }
+            m = x[h][2]; while (m) { const uint32_t b = __ffs(m) - 1u; m &= m - 1u; gout[off++] = (uint16_t)(base + 64u + b); }
+            m = x[h][3]; while (m) { const uint32_t b = __ffs(m) - 1u; m &= m - 1u; gout[off++] = (uint16_t)(base + 96u + b); }
+        }
         if (tid == 0) {
             const uint32_t lvl = runs <= 124u ? 0u : runs <= 252u ? 1u : runs <= 508u ? 2u : 3u;   // gap_calc_level src/bmfunc.h:5418
             gout[runs] = 65535u;
-            gout[0] = (uint16_t)((R.x & 1u) | (lvl << 1) | (runs << 3));
+            gout[0] = (uint16_t)((R[0].x & 1u) | (lvl << 1) | (runs << 3));
         }
     }
     if (tid == 0) {
@@ -561,6 +590,12 @@ __device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, u
         p.kind[col]   = (uint8_t)kd;
         if (tpc) atomicAdd(p.total + grp, (unsigned long long)tpc);
     }
+}
+template <bool EMPTY_DIGEST_IS_NULL, bool PIPE = false>
+__device__ __forceinline__ void finish_block(const AggParams& p, uint32_t col, uint32_t colx, uint32_t grp, uint4 R, int state,
+                                             uint32_t* K, uint32_t* s_pc, uint32_t* s_tr, uint32_t* s_dg, uint32_t rule = 0u)
+{
+    finish_block<EMPTY_DIGEST_IS_NULL, PIPE, 4>(p, col, colx, grp, Quads<1>{{R}}, state, K, s_pc, s_tr, s_dg, rule);
 }
 
 // AND / AND-SUB result state (0 = NULL, 1 = FULL, 2 = computed): an AND-group NULL block, an empty AND group or a SUB-group FULL
@@ -996,9 +1031,11 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
 // every block of column nb is needed: its bit-blocks are the contiguous run bit_pool[bit_base[nb] .. bit_base[nb+1]) and its GAP
 // blocks the contiguous units gap_pool[gap_base[nb] .. gap_base[nb+1]).  No member list has to be resolved before the bytes can be
 // requested, so one producer warp streams columns back to back with cp.async.bulk into a ring of 8 KB stages (full / empty mbarrier
-// per stage) and HBM keeps ~kPipeStages x 8 KB per SM in flight across column boundaries, while 16 consumer warps classify the
+// per stage) and HBM keeps ~kPipeStages x 8 KB per CTA in flight across column boundaries, while 8 consumer warps classify the
 // column from its descriptor row, fold the staged bit-blocks (stage j = bit-block j of the segment) and sweep the staged GAP segment
-// in FLAT form.  A column whose GAP blocks are not all FLAT SUB-group blocks (raw GAP form, GAP blocks in the AND group) releases
+// in FLAT form.  Two CTAs are resident per SM: the phases of a column are limited by different resources (the bit phase by HBM,
+// the companion sweep by shared-memory issue, classification and epilogue by barriers and latency), so while one CTA sweeps or
+// finishes a column, the other's ring keeps the SM's share of HBM busy.  A column whose GAP blocks are not all FLAT SUB-group blocks (raw GAP form, GAP blocks in the AND group) releases
 // its GAP stages unread and applies its GAP blocks straight from global memory.  With the run-list companion (RunLists, passed only
 // when the AND group holds no GAP block) the producer streams the column's companion singles and long runs in place of its GAP segment:
 // part A (the GAP blocks' runs), or A + B (also the runs of the listed bit-blocks, which it then does not stream) when the AND group
@@ -1006,26 +1043,31 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
 // Protocol (no wait can outlive the producer): the producer claims a column only when a queue slot is free, publishes (item, #bit
 // stages, GAP bytes, first stage) and then issues all of the column's stages in order, each after its empty barrier; after the last
 // column it publishes an end marker.  Consumers read every queue entry and wait for exactly the stages it announces: every warp
-// waits for every bit stage (one 16-byte word per thread); GAP or companion stage g of the column goes to the kPipeGroup warps of
+// waits for every bit stage (two 16-byte words per thread); GAP or companion stage g of the column goes to the kPipeGroup warps of
 // group g % kPipeGroups, each sweeping its kPipeSlice bytes of it.  Every waiter arrives once on the stage's empty barrier, for
-// 16 / (its waiters) warps, so a stage is free as soon as its slowest slice is done and the rest of the ring stays requested.
+// kPipeWarps / (its waiters) warps, so a stage is free as soon as its slowest slice is done and the rest of the ring stays requested.
 // They free the queue slot once the column is classified, because classification reads the column's listed flags that the
 // producer staged with the entry.  With part B the entry's bit stages are the column's unlisted bit-blocks in order.
 // Parity waits are sound because every waiter has waited for every earlier fill of the stage: fills of earlier columns all
 // completed before the column barriers the waiter has passed, and within a column a ring slot is reused only by bit stages,
-// which every warp waits for, or by GAP stages of the same warp group (kPipeStages is a multiple of kPipeGroups).
-constexpr int      kPipeStages  = 16;                      // 128 KB of stages
+// which every warp waits for, or by GAP stages of the same warp group (kPipeStages = 8 is a multiple of kPipeGroups = 4).
+constexpr int      kPipeCtasPerSm = 2;                     // resident CTAs per SM the kernel is shaped for (<= 112 registers)
+constexpr int      kPipeConsumers = 256;                   // consumer threads: 8 words of L per thread, as two uint4
+constexpr int      kPipeWarps   = kPipeConsumers / 32;
+constexpr int      kPipeWpt     = (int)kBlockWords / kPipeConsumers;
+constexpr int      kPipeStages  = 8;                       // 64 KB of stages per CTA, 128 KB per SM
 constexpr uint32_t kPipeStage   = 8192u;
-constexpr uint32_t kPipeGroup   = 2u;                      // consumer warps that share one GAP or companion stage (DESIGN §3.1a: 1, 4, 8, 16 were slower)
-constexpr uint32_t kPipeGroups  = kAggWarps / kPipeGroup;  // GAP stage g of a column goes to warp group g % kPipeGroups
+constexpr uint32_t kPipeGroup   = 2u;                      // consumer warps that share one GAP or companion stage (DESIGN §3.1a)
+constexpr uint32_t kPipeGroups  = kPipeWarps / kPipeGroup; // GAP stage g of a column goes to warp group g % kPipeGroups
 constexpr uint32_t kPipeSlice   = kPipeStage / kPipeGroup; // bytes of such a stage each warp of its group sweeps
 constexpr int      kPipeQueue   = 2;                       // columns claimed ahead of the consumers (more would unbalance the tail)
 constexpr uint32_t kPipeMaxVec  = 4096u;                   // role table size: larger sets take agg_kernel
-constexpr int      kPipePerThr  = (int)kPipeMaxVec / kAggThreads;
+constexpr int      kPipePerThr  = (int)kPipeMaxVec / kPipeConsumers;
 constexpr uint32_t kPipeMaxAndGap = 64u;                   // AND-group GAP blocks per column the FLAT path takes (more: in-place reads)
-constexpr uint32_t kPipeThreads = kAggThreads + 32u;       // 16 consumer warps + 1 producer warp
+constexpr uint32_t kPipeThreads = kPipeConsumers + 32u;    // 8 consumer warps + 1 producer warp
 constexpr size_t   kPipeRingSmem = (size_t)kPipeStages * kPipeStage;
 static_assert(kPipeStages % kPipeGroups == 0, "a ring slot must go to the same warp group each time a column reuses it");
+static_assert(kPipeWpt == 8 && kPipeStage == 2u * 16u * kPipeConsumers, "a bit stage is two LDS.128 per consumer thread");
 
 // *bad |= 1 when a GAP block of the set is not in the BMB200_DESC_GAP_FLAT form (agg_pipe_kernel sweeps SUB-group blocks as FLAT pairs)
 __global__ void desc_flat_check_kernel(const uint32_t* __restrict__ desc, size_t n, uint32_t* bad)
@@ -1050,7 +1092,7 @@ struct RunLists {
 };
 constexpr uint32_t kPipeLstWords = kPipeMaxVec / 32u;       // listed flags of one column's bit-blocks
 
-__global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggParams p, const RunLists rl)
+__global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(const AggParams p, const RunLists rl)
 {
     constexpr int OP = BMB200_OP_AND_SUB;
     extern __shared__ __align__(128) uint8_t dyn_smem[];
@@ -1069,14 +1111,14 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
     __shared__ uint32_t s_brole[2][kPipeMaxVec / 32];       // bit-block j of the column -> group1, one buffer per column parity
     __shared__ uint32_t s_st[2][6];                         // flags, bit0, gap0, AND-group GAP blocks, non-FLAT, first GAP unit
     __shared__ uint2 s_ag[2][kPipeMaxAndGap];               // AND-group GAP blocks of the column: (descriptor, end of its last 16-byte unit)
-    __shared__ uint32_t s_pc[kAggWarps], s_tr[kAggWarps], s_dg[kAggWarps];
+    __shared__ uint32_t s_pc[kPipeWarps], s_tr[kPipeWarps], s_dg[kPipeWarps];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t M = p.set.n_vec;
     const uint32_t n0 = p.goff[1], n1 = p.goff[2] - p.goff[1];
     if (tid == 0) {
-        for (int s = 0; s < kPipeStages; ++s) { mbar_init(&s_full[s], 1u); mbar_init(&s_empty[s], kAggWarps); }
-        for (int q = 0; q < kPipeQueue; ++q) { mbar_init(&s_qfull[q], 1u); mbar_init(&s_qempty[q], kAggWarps); }
+        for (int s = 0; s < kPipeStages; ++s) { mbar_init(&s_full[s], 1u); mbar_init(&s_empty[s], kPipeWarps); }
+        for (int q = 0; q < kPipeQueue; ++q) { mbar_init(&s_qfull[q], 1u); mbar_init(&s_qempty[q], kPipeWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (uint32_t i = tid; i < kPipeMaxVec / 32; i += kPipeThreads) { s_g1[i] = 0u; s_brole[0][i] = 0u; }
@@ -1085,7 +1127,7 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
     for (uint32_t k = n0 + tid; k < n0 + n1; k += kPipeThreads) { const uint32_t v = p.group[k]; atomicOr(&s_g1[v >> 5], 1u << (v & 31u)); }
     __syncthreads();                                        // the last CTA-wide barrier: the producer warp leaves below
 
-    if (warp == kAggWarps) {                                // ---- producer (one lane) ----
+    if (warp == kPipeWarps) {                               // ---- producer (one lane) ----
         if (lane != 0) return;
         uint32_t seq = 0;
         for (uint32_t qi = 0;; ++qi) {
@@ -1141,14 +1183,14 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
         }
     }
 
-    // ---- consumers: tid < kAggThreads ----
+    // ---- consumers: tid < kPipeConsumers; thread t holds words [4t, 4t + 4) and [4 (t + 256), 4 (t + 256) + 4) of L ----
     uint4* K4 = reinterpret_cast<uint4*>(K);
     uint32_t Ks, ring_s;
     asm volatile("mov.u32 %0, %1;" : "=r"(Ks) : "r"(smem_u32(K)));
     asm volatile("mov.u32 %0, %1;" : "=r"(ring_s) : "r"(smem_u32(ring)));
+    constexpr int H = kPipeWpt / 4;
     for (uint32_t qi = 0;; ++qi) {
         const uint32_t b = qi & 1u, qs = qi % kPipeQueue;
-        K4[tid] = make_uint4(~0u, ~0u, ~0u, ~0u);           // live mask: every bit still a candidate
         if (tid < 6) s_st[b ^ 1u][tid] = (tid == 5) ? ~0u : 0u;          // next column's counters (nobody reads them any more)
         if (tid < (int)(kPipeMaxVec / 32)) s_brole[b ^ 1u][tid] = 0u;
         mbar_wait(&s_qfull[qs], (qi / kPipeQueue) & 1u);
@@ -1160,48 +1202,53 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
         const uint32_t* drow = p.set.desc + (size_t)nb * M;
         const uint16_t* gseg = p.set.gap_pool + p.set.gap_base[nb] * (size_t)kGapUnit;
 
-        // ---- classification by vector (every vector is a member: no member list to resolve) ----
-        uint32_t dv[kPipePerThr];
-        uint32_t fl = 0, nb0 = 0, ng0 = 0, nonflat = 0, lo = ~0u;
+        // ---- classification by vector (every vector is a member: no member list to resolve); vector tid + 256 i is trip i ----
+        // The descriptors are dropped after it: the rare paths behind the bit phase re-read the row.  `lead` keeps the one fact
+        // the FLAT path needs from it, bit i = trip i's vector is a SUB-group GAP block without lead pad.
+        uint32_t fl = 0, nb0 = 0, ng0 = 0, nonflat = 0, lo = ~0u, lead = 0;
+        {
+            uint32_t dv[kPipePerThr];
 #pragma unroll
-        for (int i = 0; i < kPipePerThr; ++i) {
-            const uint32_t v = (uint32_t)tid + (uint32_t)i * kAggThreads;
-            dv[i] = v < M ? drow[v] : BMB200_BLK_NULL;
-        }
+            for (int i = 0; i < kPipePerThr; ++i) {
+                const uint32_t v = (uint32_t)tid + (uint32_t)i * kPipeConsumers;
+                dv[i] = v < M ? drow[v] : BMB200_BLK_NULL;
+            }
 #pragma unroll
-        for (int i = 0; i < kPipePerThr; ++i) {
-            const uint32_t v = (uint32_t)tid + (uint32_t)i * kAggThreads;
-            if (v >= M) continue;
-            const uint32_t d = dv[i], kind = d & 3u;
-            const bool g1 = (s_g1[v >> 5] >> (v & 31u)) & 1u;
-            if (kind == BMB200_BLK_BIT) {
-                // role by streamed index: rel minus the listed blocks below it (a listed block is a SUB-group block, never streamed)
-                if (g1) {
-                    uint32_t j = (d >> 2) & (kPipeMaxVec - 1u);
-                    if (rl.listed) {
-                        const uint32_t f = s_lst[qs][j >> 5], below = f & ((1u << (j & 31u)) - 1u);
-                        if ((f >> (j & 31u)) & 1u) continue;
-                        j -= s_lrk[qs][j >> 5] + __popc(below);
+            for (int i = 0; i < kPipePerThr; ++i) {
+                const uint32_t v = (uint32_t)tid + (uint32_t)i * kPipeConsumers;
+                if (v >= M) continue;
+                const uint32_t d = dv[i], kind = d & 3u;
+                const bool g1 = (s_g1[v >> 5] >> (v & 31u)) & 1u;
+                if (kind == BMB200_BLK_BIT) {
+                    // role by streamed index: rel minus the listed blocks below it (a listed block is a SUB-group block, never streamed)
+                    if (g1) {
+                        uint32_t j = (d >> 2) & (kPipeMaxVec - 1u);
+                        if (rl.listed) {
+                            const uint32_t f = s_lst[qs][j >> 5], below = f & ((1u << (j & 31u)) - 1u);
+                            if ((f >> (j & 31u)) & 1u) continue;
+                            j -= s_lrk[qs][j >> 5] + __popc(below);
+                        }
+                        atomicOr(&s_brole[b][j >> 5], 1u << (j & 31u));
+                    } else {
+                        ++nb0;
                     }
-                    atomicOr(&s_brole[b][j >> 5], 1u << (j & 31u));
+                } else if (kind == BMB200_BLK_GAP) {
+                    const uint32_t u = (d >> 2) & kRelMask;
+                    if (g1) {
+                        if (!((d >> 2) & kEntFlat)) nonflat = 1u;         // the FLAT sweep reads SUB-group blocks in FLAT form only
+                        if (!(d >> 31)) lead |= 1u << i;
+                    } else {                                              // AND group: listed, applied from global memory and blanked in the stage
+                        ++ng0;
+                        const uint32_t k = atomicAdd(&s_st[b][3], 1u);
+                        if (k < kPipeMaxAndGap) s_ag[b][k] = make_uint2(d, (u * 16u + 2u * (d >> 31) + 2u * ((gseg[(size_t)u * kGapUnit + (d >> 31)] >> 3) + 1u) + 15u) & ~15u);
+                        else nonflat = 1u;
+                    }
+                    lo = min(lo, u);
+                } else if (kind == BMB200_BLK_NULL) {
+                    if (!g1) fl |= kFlNull0;
                 } else {
-                    ++nb0;
+                    fl |= g1 ? kFlFull1 : kFlFull0;
                 }
-            } else if (kind == BMB200_BLK_GAP) {
-                const uint32_t u = (d >> 2) & kRelMask;
-                if (g1) {
-                    if (!((d >> 2) & kEntFlat)) nonflat = 1u;         // the FLAT sweep reads SUB-group blocks in FLAT form only
-                } else {                                              // AND group: listed, applied from global memory and blanked in the stage
-                    ++ng0;
-                    const uint32_t k = atomicAdd(&s_st[b][3], 1u);
-                    if (k < kPipeMaxAndGap) s_ag[b][k] = make_uint2(d, (u * 16u + 2u * (d >> 31) + 2u * ((gseg[(size_t)u * kGapUnit + (d >> 31)] >> 3) + 1u) + 15u) & ~15u);
-                    else nonflat = 1u;
-                }
-                lo = min(lo, u);
-            } else if (kind == BMB200_BLK_NULL) {
-                if (!g1) fl |= kFlNull0;
-            } else {
-                fl |= g1 ? kFlFull1 : kFlFull0;
             }
         }
         fl = __reduce_or_sync(0xffffffffu, fl); nonflat = __reduce_or_sync(0xffffffffu, nonflat); lo = __reduce_min_sync(0xffffffffu, lo);
@@ -1213,29 +1260,33 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
             if (nonflat) s_st[b][4] = 1u;
             if (lo != ~0u) atomicMin(&s_st[b][5], lo);
         }
-        agg_sync<true>();
+        agg_sync<true, kPipeConsumers>();
         if (lane == 0) mbar_arrive(&s_qempty[qs]);               // the entry and its listed flags are read: the slot may be refilled
         // FLAT: the whole GAP segment is a flat window of 1-run sources (headers, pads and tail fill decode to empty runs)
         const bool flat = s_st[b][4] == 0u && s_st[b][5] == 0u;
         const uint32_t nag = s_st[b][3];                         // <= kPipeMaxAndGap when flat
 
-        // ---- bit phase: stage j = bit-block j of the column ----
-        uint4 acc0 = make_uint4(~0u, ~0u, ~0u, ~0u);
-        uint4 acc1 = make_uint4(0u, 0u, 0u, 0u);
+        // ---- bit phase: stage j = bit-block j of the column, two LDS.128 per thread ----
+        uint4 acc0[H], acc1[H];
+#pragma unroll
+        for (int h = 0; h < H; ++h) { acc0[h] = make_uint4(~0u, ~0u, ~0u, ~0u); acc1[h] = make_uint4(0u, 0u, 0u, 0u); }
         for (uint32_t j = 0; j < nbit; ++j) {
             const uint32_t sq = seq0 + j, s = sq % kPipeStages;
             mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
-            const uint4 v = lds128(ring_s + s * kPipeStage + (uint32_t)tid * 16u);
-            if ((s_brole[b][j >> 5] >> (j & 31u)) & 1u) acc_or(acc1, v); else acc_apply0<OP>(acc0, v);
+            uint4 v[H];
+#pragma unroll
+            for (int h = 0; h < H; ++h) v[h] = lds128(ring_s + s * kPipeStage + (uint32_t)(h * kPipeConsumers + tid) * 16u);
+            const bool sub = (s_brole[b][j >> 5] >> (j & 31u)) & 1u;
+#pragma unroll
+            for (int h = 0; h < H; ++h) { if (sub) acc_or(acc1[h], v[h]); else acc_apply0<OP>(acc0[h], v[h]); }
             __syncwarp();
             if (lane == 0) mbar_arrive(&s_empty[s]);
         }
-        {
-            uint4 l = K4[tid];
-            l.x &= acc0.x & ~acc1.x; l.y &= acc0.y & ~acc1.y; l.z &= acc0.z & ~acc1.z; l.w &= acc0.w & ~acc1.w;
-            K4[tid] = l;
-        }
-        agg_sync<true>();
+        // live mask L = AND of the AND-group bit-blocks minus the SUB-group ones (every bit a candidate without bit-blocks)
+#pragma unroll
+        for (int h = 0; h < H; ++h)
+            K4[h * kPipeConsumers + tid] = make_uint4(acc0[h].x & ~acc1[h].x, acc0[h].y & ~acc1[h].y, acc0[h].z & ~acc1[h].z, acc0[h].w & ~acc1[h].w);
+        agg_sync<true, kPipeConsumers>();
 
         // ---- GAP phase: GAP stage g goes to warp group g % kPipeGroups; a warp sweeps bytes [wlo, wlo + kPipeSlice) of it ----
         const uint32_t ngs = (gbytes + kPipeStage - 1u) / kPipeStage;
@@ -1259,13 +1310,11 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
             }
         } else if (flat) {
             // a FLAT SUB-group block without lead pad starts with a 1-run whose pair slot holds the header: clear that whole run here
-#pragma unroll
-            for (int i = 0; i < kPipePerThr; ++i) {
-                const uint32_t d = dv[i], v = (uint32_t)tid + (uint32_t)i * kAggThreads;
-                if (v < M && (d & 3u) == BMB200_BLK_GAP && !(d >> 31) && ((s_g1[v >> 5] >> (v & 31u)) & 1u))
-                    apply_run<false>(Ks, 0u, gseg[(size_t)((d >> 2) & kRelMask) * kGapUnit + 1u]);
+            for (uint32_t m = lead; m; m &= m - 1u) {
+                const uint32_t v = (uint32_t)tid + (uint32_t)(__ffs(m) - 1) * kPipeConsumers;
+                apply_run<false>(Ks, 0u, gseg[(size_t)((drow[v] >> 2) & kRelMask) * kGapUnit + 1u]);
             }
-            for (uint32_t i = (uint32_t)warp; i < nag; i += kAggWarps) {   // AND-group GAP blocks: their 0-runs, read in place
+            for (uint32_t i = (uint32_t)warp; i < nag; i += kPipeWarps) {  // AND-group GAP blocks: their 0-runs, read in place
                 const uint32_t d = s_ag[b][i].x;
                 gap_scatter_gather<false>(Ks, gseg + (size_t)((d >> 2) & kRelMask) * kGapUnit + (d >> 31), 0u, lane);
             }
@@ -1296,25 +1345,28 @@ __global__ void __launch_bounds__(kPipeThreads, 1) agg_pipe_kernel(const AggPara
                 mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
                 if (lane == 0) mbar_arrive(&s_empty[s]);
             }
-#pragma unroll
-            for (int i = 0; i < kPipePerThr; ++i) {            // this warp's 32 vectors of trip i, one GAP block at a time
-                const uint32_t v = (uint32_t)tid + (uint32_t)i * kAggThreads;
-                uint32_t m = __ballot_sync(0xffffffffu, v < M && (dv[i] & 3u) == BMB200_BLK_GAP);
+            for (int i = 0; i < kPipePerThr; ++i) {                   // this warp's 32 vectors of trip i, one GAP block at a time
+                const uint32_t v = (uint32_t)tid + (uint32_t)i * kPipeConsumers;
+                const uint32_t dv = v < M ? drow[v] : BMB200_BLK_NULL;
+                uint32_t m = __ballot_sync(0xffffffffu, (dv & 3u) == BMB200_BLK_GAP);
                 while (m) {
                     const int l = __ffs(m) - 1; m &= m - 1u;
-                    const uint32_t d = __shfl_sync(0xffffffffu, dv[i], l);
+                    const uint32_t d = __shfl_sync(0xffffffffu, dv, l);
                     const uint32_t vl = v - (uint32_t)lane + (uint32_t)l;
                     const uint32_t want = (s_g1[vl >> 5] >> (vl & 31u)) & 1u;   // AND group: 0-runs, SUB group: 1-runs
                     gap_scatter_gather<false>(Ks, gseg + (size_t)((d >> 2) & kRelMask) * kGapUnit + (d >> 31), want, lane);
                 }
             }
         }
-        agg_sync<true>();
+        agg_sync<true, kPipeConsumers>();
 
         // ---- epilogue ----
         const int state = and_state<OP>(s_st[b][0], s_st[b][1], s_st[b][2], n0, n1);
-        const uint4 R = state == 0 ? make_uint4(0u, 0u, 0u, 0u) : state == 1 ? make_uint4(~0u, ~0u, ~0u, ~0u) : K4[tid];
-        finish_block<true, true>(p, item, item, 0u, R, state, K, s_pc, s_tr, s_dg);
+        Quads<H> R;
+#pragma unroll
+        for (int h = 0; h < H; ++h)
+            R.q[h] = state == 0 ? make_uint4(0u, 0u, 0u, 0u) : state == 1 ? make_uint4(~0u, ~0u, ~0u, ~0u) : K4[h * kPipeConsumers + tid];
+        finish_block<true, true, kPipeWpt>(p, item, item, 0u, R, state, K, s_pc, s_tr, s_dg);
     }
 }
 

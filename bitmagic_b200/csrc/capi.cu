@@ -82,6 +82,7 @@ struct bmb200_ctx {
     bool attr_set = false, merge_attr_set = false;
     size_t agg_dyn[4] = {};                 // dynamic shared memory per agg_kernel<OP> (set_agg_attrs)
     size_t pipe_dyn = 0;                    // ... of agg_pipe_kernel
+    int pipe_ctas_per_sm = 1;               // resident agg_pipe_kernel CTAs per SM with that shared memory (occupancy query)
     int agg_pipeline = 1;                   // 1 = whole-set AND-SUB takes agg_pipe_kernel, 0 = always agg_kernel
     int run_lists = 1;                      // run-list companion of agg_pipe_kernel: 0 never, 1 from a set's second qualifying call, 2 from its first
     int host_threads = 0;                   // host threads of bmb200_set_upload_vectors (0 = hardware concurrency, at most 64)
@@ -1220,6 +1221,10 @@ static void set_agg_attrs(bmb200_ctx* ctx, cudaError_t* e)
     *e = cudaSuccess;
     for (int op = 0; op < 4 && *e == cudaSuccess; ++op) *e = agg_attr_one(kAggKernels[op], (size_t)reserved, &ctx->agg_dyn[op]);
     if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel, (size_t)reserved, &ctx->pipe_dyn, kPipeRingSmem);
+    // the kernel is shaped for kPipeCtasPerSm CTAs per SM; its grid follows what the device actually grants (at least one)
+    if (*e == cudaSuccess)
+        *e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->pipe_ctas_per_sm, agg_pipe_kernel, (int)kPipeThreads, ctx->pipe_dyn);
+    if (*e == cudaSuccess && ctx->pipe_ctas_per_sm < 1) ctx->pipe_ctas_per_sm = 1;
     if (*e == cudaSuccess) ctx->attr_set = true;
 }
 
@@ -1469,11 +1474,12 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     RunLists rl{};
     if (ctx->agg_pipeline && ctx->gap_mode == 0 && set->n_gap_units && whole_set(a, set->v.n_vec) &&
         (use_run_lists(ctx, set, a, &rl) || flat_gap_set(ctx, set))) {
-        // one AND-SUB group naming every vector once: a producer warp streams whole columns (agg_pipe_kernel), one CTA per SM,
-        // with the GAP segments or the run-list companion behind the bit-blocks.
+        // one AND-SUB group naming every vector once: a producer warp per CTA streams whole columns (agg_pipe_kernel), two CTAs
+        // per SM, with the GAP segments or the run-list companion behind the bit-blocks.
         // OR stays on agg_kernel: its whole-set workloads measured at par or slower through the ring (DESIGN §3.1a)
         p.dyn_bytes = (uint32_t)ctx->pipe_dyn;
-        const uint32_t pgrid = sms < n_cols ? sms : n_cols;
+        const uint32_t pctas = sms * (uint32_t)ctx->pipe_ctas_per_sm;
+        const uint32_t pgrid = pctas < n_cols ? pctas : n_cols;
         agg_pipe_kernel<<<pgrid, kPipeThreads, ctx->pipe_dyn, ctx->stream>>>(p, rl);
     } else if (a->op == BMB200_OP_SHIFT_R_AND) {
         shift_and_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p);

@@ -22,9 +22,10 @@ namespace bmb200 {
 constexpr int kRlThreads = 512;
 constexpr int kRlWarps   = kRlThreads / 32;
 // A bit-block is listed when 2 x singles + 4 x long runs <= kListBitMax bytes.  Every listed run is one more position for the
-// consumers to sweep, so a larger threshold streams fewer bytes but sweeps more.  On C3 (H100 80GB HBM3, 400 W, DESIGN §6) the
-// whole-set AND-SUB took 3.26 / 3.07 / 3.20 / 3.56 / 3.80 ms at 2048 / 3072 / 4096 / 6144 / 8192: 3072 is the fastest.
-constexpr uint32_t kListBitMax = 3072u;
+// consumers to sweep, so a larger threshold streams fewer bytes but sweeps more.  With one CTA per SM (H100 80GB HBM3, 400 W,
+// DESIGN §6) C3 took 3.26 / 3.07 / 3.20 / 3.56 / 3.80 ms at 2048 / 3072 / 4096 / 6144 / 8192; with two CTAs per SM, whose sweeps
+// overlap the other CTA's stream, 4096 is the faster of 3072 / 4096 (2.20 against 2.29 ms at 700 W).
+constexpr uint32_t kListBitMax = 4096u;
 
 // One warp decodes the GAP block at g (= &buf[0], lead pad already skipped) and appends its 1-runs in order: singles to sout[ns..),
 // long-run pairs to lout[nl..) (WRITE), or only counts them.  ns / nl are warp-uniform running counts.
