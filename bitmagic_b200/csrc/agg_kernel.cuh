@@ -302,27 +302,17 @@ __device__ __forceinline__ void flat_quad(uint32_t Ls, const uint4& q)
     if (reach > 32u) flat_quad_tail(Ls, q);
 }
 
-// Singles of the run-list companion (runlist_kernel.cuh): eight u16 bit positions per 128-bit load, one bit each.
-// MODE 0: one atomic per position.  MODE 1: test-first, as in flat_quad.
-template <int MODE>
+// Singles of the run-list companion (runlist_kernel.cuh): eight u16 bit positions per 128-bit load, one bit each, one atomic per
+// position.  The singles are dealt out by bank, so a warp's atomic is one shared-memory wavefront in a part's full rounds, and a
+// test-first form (`lds32`, then a predicated atomic, as flat_quad's MODE 1) only adds a dependent shared-memory round trip per
+// position: it was 0.9 % slower on C3 (2.202-2.205 against 2.182 ms, H100 80GB HBM3 at 700 W), where L is 12 % alive and less.
 __device__ __forceinline__ void sgl_oct(uint32_t Ls, const uint4& q)
 {
     const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-    uint32_t a[8], m[8];
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-        a[2 * i]     = and_or(w[i] >> 3, 0x1ffcu, Ls);  m[2 * i]     = 1u << (w[i] & 31u);
-        a[2 * i + 1] = and_or(w[i] >> 19, 0x1ffcu, Ls); m[2 * i + 1] = 1u << ((w[i] >> 16) & 31u);
-    }
-    if (MODE) {
-        uint32_t v[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = lds32(a[i]) & m[i];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) reds_and_if(a[i], ~m[i], v[i]);
-    } else {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) reds_and(a[i], ~m[i]);
+        reds_and(and_or(w[i] >> 3, 0x1ffcu, Ls), ~(1u << (w[i] & 31u)));
+        reds_and(and_or(w[i] >> 19, 0x1ffcu, Ls), ~(1u << ((w[i] >> 16) & 31u)));
     }
 }
 
@@ -333,7 +323,7 @@ __device__ __forceinline__ void sgl_oct(uint32_t Ls, const uint4& q)
 template <int MODE, bool SGL = false>
 __device__ __forceinline__ void flat_sweep_mode(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off)
 {
-    auto eat = [&](const uint4& q) { if (SGL) sgl_oct<MODE>(Ls, q); else flat_quad<MODE>(Ls, q); };
+    auto eat = [&](const uint4& q) { if (SGL) sgl_oct(Ls, q); else flat_quad<MODE>(Ls, q); };
     uint32_t h = 0;
 #pragma unroll 1
     for (; h + 1024u <= bytes; h += 1024u) {
@@ -347,9 +337,9 @@ __device__ __noinline__ void flat_sweep_fn(uint32_t Ls, uint32_t src, uint32_t b
 {
     if (mode) flat_sweep_mode<1>(Ls, src, bytes, lane_off); else flat_sweep_mode<0>(Ls, src, bytes, lane_off);
 }
-__device__ __noinline__ void sgl_sweep_fn(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off, uint32_t mode)
+__device__ __noinline__ void sgl_sweep_fn(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off)
 {
-    if (mode) flat_sweep_mode<1, true>(Ls, src, bytes, lane_off); else flat_sweep_mode<0, true>(Ls, src, bytes, lane_off);
+    flat_sweep_mode<0, true>(Ls, src, bytes, lane_off);
 }
 // The sweep's form for one column, re-sampled before each piece until it switches (warp-uniform): a 1024-bit sample of L (piece
 // number c varies the sample); below 25 % alive the test-first form wins (one shared load, rarely an atomic).  Bits of L only ever
@@ -1050,12 +1040,12 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
 // producer staged with the entry.  With part B the entry's bit stages are the column's unlisted bit-blocks in order.
 // Parity waits are sound because every waiter has waited for every earlier fill of the stage: fills of earlier columns all
 // completed before the column barriers the waiter has passed, and within a column a ring slot is reused only by bit stages,
-// which every warp waits for, or by GAP stages of the same warp group (kPipeStages = 8 is a multiple of kPipeGroups = 4).
+// which every warp waits for, or by GAP stages of the same warp group (kPipeStages = 12 is a multiple of kPipeGroups = 4).
 constexpr int      kPipeCtasPerSm = 2;                     // resident CTAs per SM the kernel is shaped for (<= 112 registers)
 constexpr int      kPipeConsumers = 256;                   // consumer threads: 8 words of L per thread, as two uint4
 constexpr int      kPipeWarps   = kPipeConsumers / 32;
 constexpr int      kPipeWpt     = (int)kBlockWords / kPipeConsumers;
-constexpr int      kPipeStages  = 8;                       // 64 KB of stages per CTA, 128 KB per SM
+constexpr int      kPipeStages  = 12;                      // 96 KB of stages per CTA: with L and the static part 112 KB, so two CTAs fill the SM's 228 KB
 constexpr uint32_t kPipeStage   = 8192u;
 constexpr uint32_t kPipeGroup   = 2u;                      // consumer warps that share one GAP or companion stage (DESIGN §3.1a)
 constexpr uint32_t kPipeGroups  = kPipeWarps / kPipeGroup; // GAP stage g of a column goes to warp group g % kPipeGroups
@@ -1302,9 +1292,12 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
                 const uint32_t bytes = sgl ? min(kPipeStage, gbytes - g * kPipeStage) : min(kPipeStage, lbytes - (g - ngs) * kPipeStage);
                 const uint32_t src = ring_s + s * kPipeStage + wlo + (uint32_t)lane * 16u, sb = bytes > wlo ? bytes - wlo : 0u;
                 mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
-                flat_update_mode(flat_mode, Ks, (uint32_t)lane, g);
-                if (sgl) sgl_sweep_fn(Ks, src, min(kPipeSlice, sb), (uint32_t)lane * 16u, flat_mode);      // a partial last stage
-                else     flat_sweep_fn(Ks, src, min(kPipeSlice, sb), (uint32_t)lane * 16u, flat_mode);     // leaves later slices empty
+                if (sgl) {
+                    sgl_sweep_fn(Ks, src, min(kPipeSlice, sb), (uint32_t)lane * 16u);                      // a partial last stage
+                } else {                                                                                   // leaves later slices empty
+                    flat_update_mode(flat_mode, Ks, (uint32_t)lane, g);
+                    flat_sweep_fn(Ks, src, min(kPipeSlice, sb), (uint32_t)lane * 16u, flat_mode);
+                }
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&s_empty[s], kPipeGroups);
             }

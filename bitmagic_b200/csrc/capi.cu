@@ -1345,7 +1345,7 @@ static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
     uint2* wcnt = nullptr; uint64_t *su = nullptr, *lu = nullptr; unsigned long long* tot = nullptr; uint32_t* lv = nullptr;
     uint64_t h_tot[5] = {0, 0, 0, 0, 0};
     std::vector<uint32_t> h_lv(vwords, 0u);
-    bool ok = cudaMalloc((void**)&wcnt, (size_t)nb * 2 * kRlWarps * sizeof(uint2)) == cudaSuccess &&
+    bool ok = cudaMalloc((void**)&wcnt, (size_t)nb * kRlCnt * sizeof(uint2)) == cudaSuccess &&
               cudaMalloc((void**)&su, (size_t)nb * 8) == cudaSuccess && cudaMalloc((void**)&lu, (size_t)nb * 8) == cudaSuccess &&
               cudaMalloc((void**)&tot, sizeof(h_tot)) == cudaSuccess && cudaMalloc((void**)&lv, vwords * 4u) == cudaSuccess &&
               cudaMalloc((void**)&s->rl_sgl_base, ((size_t)nb + 1) * 8) == cudaSuccess &&
