@@ -4,7 +4,7 @@ Product code: csrc/ (CUDA kernels + the C ABI of include/bmb200.h, built into li
 host-side mirror of the reference operator surface (aggregator.py, scanner.py, hostfmt.py, capi.py).
 There is no CPU fallback: importing works anywhere, computing needs libbmb200.so and an H100.
 """
-from .capi import (BLK_BIT, BLK_FULL, BLK_GAP, BLK_NULL, F_COUNT_ONLY, F_OPT_COMPRESS, F_OPT_NONE, F_OR_TARGET, OP_AND,
+from .capi import (BLK_BIT, BLK_FULL, BLK_GAP, BLK_NULL, F_COUNT_ONLY, F_OPT_COMPRESS, F_OPT_NONE, F_OR_TARGET, F_SIGNED, OP_AND,
                    OP_AND_SUB, OP_OR, OP_XOR, OP_SHIFT_R_AND, BMB200Error, Context, DeviceResult, DeviceRS, DeviceSet,
                    aggregate, aggregate_batch, aggregate_host, default_context, scan, rank_compress, rank_decompress,
                    SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT, SCAN_RANGE, NO_UNIVERSE)

@@ -23,6 +23,7 @@ GAP_MAX_WORDS, GAP_THRESHOLD, GAP_UNIT_WORDS, SUPERBLOCK = 1280, 1276, 8, 256
 BLK_NULL, BLK_FULL, BLK_BIT, BLK_GAP = 0, 1, 2, 3
 OP_OR, OP_AND, OP_AND_SUB, OP_XOR, OP_SHIFT_R_AND = 0, 1, 2, 3, 4
 F_COUNT_ONLY, F_OPT_NONE, F_OPT_COMPRESS, F_OR_TARGET = 1, 0, 2, 4
+F_SIGNED = 8                  # bmb200_scan: s2u planes (plane0 = sign plane), int64 search values
 
 # every symbol include/bmb200.h declares (checked by tests/test_cabi_symbols.py)
 SYMBOLS = [
@@ -545,8 +546,12 @@ def aggregate_batch(ctx: Context, dset: DeviceSet, op: int, groups, flags: int =
 def scan(ctx: Context, dset: DeviceSet, pred: int, values, plane0: int, n_planes: int, universe: int = NO_UNIVERSE,
          flags: int = 0, nb_from: int = 0, nb_to: int = 0, result: DeviceResult | None = None) -> DeviceResult:
     """bmb200_scan: bit-sliced comparison of the sparse vector whose plane j is set vector plane0 + j against every search
-    value (SCAN_RANGE: rows of (lo, hi)); the result has n_values * n_cols columns, value-major."""
-    vals = np.ascontiguousarray(values, dtype=np.uint64)
+    value (SCAN_RANGE: rows of (lo, hi)); the result has n_values * n_cols columns, value-major.  With F_SIGNED in flags
+    the values are signed (int64) and plane0 is the sign plane of s2u-encoded elements."""
+    if int(flags) & F_SIGNED:
+        vals = np.ascontiguousarray(np.asarray(values, np.int64).view(np.uint64))
+    else:
+        vals = np.ascontiguousarray(values, dtype=np.uint64)
     nv = vals.shape[0] if pred == SCAN_RANGE else vals.size
     if pred == SCAN_RANGE and (vals.ndim != 2 or vals.shape[1] != 2):
         raise ValueError("SCAN_RANGE takes an array of (lo, hi) rows")

@@ -1598,7 +1598,10 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
     const uint64_t items = (uint64_t)cols * ((nv + vg - 1) / vg);
     uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
     if (grid > items) grid = (uint32_t)items;
-    #define BMB200_SCAN_LAUNCH(VG, MODE) scan_kernel<VG, MODE><<<grid, kAggThreads, 0, ctx->stream>>>(sp)
+    // BMB200_F_SIGNED selects the signed instantiations (s2u planes, int64 values) with the same launch shapes
+    #define BMB200_SCAN_LAUNCH(VG, MODE) \
+        do { if (a->flags & BMB200_F_SIGNED) scan_kernel<VG, MODE, true><<<grid, kAggThreads, 0, ctx->stream>>>(sp); \
+             else scan_kernel<VG, MODE><<<grid, kAggThreads, 0, ctx->stream>>>(sp); } while (0)
     if (mode == 0)      { if (vg == 4) BMB200_SCAN_LAUNCH(4, 0); else if (vg == 2) BMB200_SCAN_LAUNCH(2, 0); else BMB200_SCAN_LAUNCH(1, 0); }
     else if (mode == 1) { if (vg == 2) BMB200_SCAN_LAUNCH(2, 1); else BMB200_SCAN_LAUNCH(1, 1); }
     else                { if (vg == 2) BMB200_SCAN_LAUNCH(2, 2); else BMB200_SCAN_LAUNCH(1, 2); }

@@ -1,6 +1,6 @@
 // scan_kernel.cuh -- bit-sliced comparison scan over the planes of a sparse vector (sm_90a).
 //
-// Replaces the reference's sparse_vector_scanner<SV> searches for unsigned sparse vectors
+// Replaces the reference's sparse_vector_scanner<SV> searches for unsigned and signed sparse vectors
 //   find_eq   src/bmsparsevec_algo.h:4360-4395 (prepare_and_sub_aggregator :2593-2632 + aggregator::combine_and_sub)
 //   find_gt / find_ge / find_lt / find_le / find_range   src/bmsparsevec_algo.h:1135-1182 (find_gt_horizontal & co.)
 // which the reference builds out of many aggregator / bvector passes over the planes.  Here ONE pass over the
@@ -20,6 +20,21 @@
 // Plane blocks may be NULL / FULL / bit / GAP like any other block of the set; GAP planes are expanded through the
 // 8 KB shared mask (block-wide run scatter), bit planes stream through 128-bit loads, four planes in flight.
 // The result goes through the same epilogue as the aggregation kernel (popcount, digest, run count, kind, bit->GAP).
+//
+// Signed vectors (SIGNED = true; bm::sparse_vector<int32_t / int64_t>, src/bmbmatrix.h:2536-2569) store u = s2u(x):
+// x >= 0 -> x << 1, x < 0 -> (-(x+1)) << 1 | 1, so plane 0 is the sign plane S and planes 1..n-1 hold the magnitude m
+// (a negative element is -(m+1)).  The reference answers a signed inequality with several whole-vector passes
+// (find_gt_horizontal_s, src/bmsparsevec_algo.h:3032-3219); here it is the same single pass:
+//   * the search value is staged as s2u(v): bits 1.. are the magnitude vm (v >= 0 ? v : ~v), bit 0 its sign;
+//   * the walk runs over planes n-1..1 only, giving EQm / GTm, the magnitude comparison against vm (a value with
+//     magnitude bits above the top plane starts with an empty EQ state, exactly as in the unsigned walk);
+//   * plane 0 is loaded once after the walk and combined per value:
+//         v >= 0:  EQ = EQm & ~S    GT = GTm & ~S
+//         v <  0:  EQ = EQm &  S    GT = U & ~(S & (EQm | GTm))     (non-negatives, and negatives of smaller magnitude)
+//     after which ge / lt / le / range follow from (EQ, GT) as for unsigned vectors.
+// find_eq (MODE 0) needs no sign combination: it walks all n planes against s2u(v), which is the exact equality of the
+// stored codes and keeps the EQ-only kernel's register footprint (no S, no per-value sign).  RANGE swaps reversed bounds by
+// signed order when the values are staged.
 #pragma once
 #include "gap_expand.cuh"
 
@@ -45,13 +60,33 @@ __device__ __forceinline__ void scan_step(uint4& eq, uint4& gt, const uint4& P, 
     }
 }
 
+// s2u (src/bmbmatrix.h:2536-2569) of a two's-complement int64 search value
+__device__ __forceinline__ uint64_t s2u(uint64_t v)
+{
+    return (int64_t)v >= 0 ? v << 1 : ((~v) << 1) | 1ull;
+}
+
+// (EQm, GTm) of the magnitude walk -> (EQ, GT) of the signed comparison, S = sign plane, neg = the value is negative
+__device__ __forceinline__ void signed_combine(uint4& e, uint4& t, const uint4& U, const uint4& S, bool neg)
+{
+    if (neg) {
+        t = make_uint4(U.x & ~(S.x & (e.x | t.x)), U.y & ~(S.y & (e.y | t.y)), U.z & ~(S.z & (e.z | t.z)), U.w & ~(S.w & (e.w | t.w)));
+        e = make_uint4(e.x & S.x, e.y & S.y, e.z & S.z, e.w & S.w);
+    } else {
+        t = make_uint4(t.x & ~S.x, t.y & ~S.y, t.z & ~S.z, t.w & ~S.w);
+        e = make_uint4(e.x & ~S.x, e.y & ~S.y, e.z & ~S.z, e.w & ~S.w);
+    }
+}
+
 // VG search values share one pass over the planes of a column (their states live side by side in registers), so plane loads
 // and GAP expansions are paid once per VG searches; RANGE keeps two state pairs per value and therefore groups fewer values.
 // MODE 0: find_eq only (no GT state), 1: one (EQ, GT) pair per value, 2: RANGE (two pairs per value)
-template <int VG, int MODE>
+// SIGNED: s2u-encoded elements, int64 search values (see the file comment)
+template <int VG, int MODE, bool SIGNED = false>
 __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const ScanParams sp)
 {
     constexpr bool RANGE = (MODE == 2), EQ_ONLY = (MODE == 0);
+    constexpr int kLowPlane = (SIGNED && !EQ_ONLY) ? 1 : 0;                  // the signed inequalities leave the sign plane out of the walk
     constexpr int kStateRegs = VG * (EQ_ONLY ? 4 : RANGE ? 16 : 8);
     constexpr int kBatch = kStateRegs > 16 ? 2 : kScanBatch;                // planes in flight: bounded by the register budget
     __shared__ __align__(16) uint32_t K[kScanBatch][kBlockWords];   // expansion buffers: the GAP planes of one batch are expanded together
@@ -86,7 +121,10 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const Sca
         if (tid < VG) {
             const uint32_t vi = min(v0 + (uint32_t)tid, p.n_groups - 1u);         // a short last group repeats its last value
             uint64_t a = sp.values[RANGE ? 2u * vi : vi], b = RANGE ? sp.values[2u * vi + 1u] : 0ull;
-            if (RANGE && b < a) { const uint64_t t = a; a = b; b = t; }           // find_range swaps reversed bounds, :2871-2872
+            if constexpr (SIGNED) {
+                if (RANGE && (int64_t)b < (int64_t)a) { const uint64_t t = a; a = b; b = t; }   // signed order, :2871-2872
+                a = s2u(a); b = s2u(b);
+            } else if (RANGE && b < a) { const uint64_t t = a; a = b; b = t; }    // find_range swaps reversed bounds, :2871-2872
             s_va[tid] = a; s_vb[tid] = b;
         }
         __syncthreads();
@@ -123,14 +161,14 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const Sca
             }
         }
 
-        for (int jt = (int)sp.n_planes - 1; jt >= 0; jt -= kBatch) {
+        for (int jt = (int)sp.n_planes - 1; jt >= kLowPlane; jt -= kBatch) {
             uint4 P[kBatch];
             uint32_t d[kBatch];
             bool any_gap = false;
 #pragma unroll
             for (int u = 0; u < kBatch; ++u) {               // issue the bit-plane loads of the batch together
                 const int j = jt - u;
-                d[u] = (j >= 0) ? s_desc[j] : BMB200_BLK_NULL;
+                d[u] = (j >= kLowPlane) ? s_desc[j] : BMB200_BLK_NULL;
                 if ((d[u] & 3u) != BMB200_BLK_GAP) P[u] = load_now(d[u]); else any_gap = true;
             }
             if (any_gap) {                                   // uniform: the GAP planes of the batch share one pair of barriers
@@ -153,7 +191,7 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const Sca
 #pragma unroll
             for (int u = 0; u < kBatch; ++u) {
                 const int j = jt - u;
-                if (j < 0) break;
+                if (j < kLowPlane) break;
 #pragma unroll
                 for (int g = 0; g < VG; ++g) {
                     if (EQ_ONLY) {
@@ -165,6 +203,15 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const Sca
             }
         }
 
+        if constexpr (kLowPlane == 1) {                      // the sign plane, folded into the states before the epilogue
+            const uint32_t ds = s_desc[0];
+            const uint4 S = ((ds & 3u) == BMB200_BLK_GAP) ? load_gap(ds) : load_now(ds);
+#pragma unroll
+            for (int g = 0; g < VG; ++g) {
+                signed_combine(eqA[g], gtA[g], U, S, s_va[g] & 1ull);
+                if (RANGE) signed_combine(eqB[RANGE ? g : 0], gtB[RANGE ? g : 0], U, S, s_vb[g] & 1ull);
+            }
+        }
 #pragma unroll
         for (int g = 0; g < VG; ++g) {
             const uint32_t vi = v0 + (uint32_t)g;

@@ -1,5 +1,6 @@
 // bmb200_scanner.hpp -- reference-side binding: bm::b200::scanner<SV>, the GPU counterpart of
-// bm::sparse_vector_scanner<SV> (src/bmsparsevec_algo.h:1040-1182) for unsigned bm::sparse_vector<>.
+// bm::sparse_vector_scanner<SV> (src/bmsparsevec_algo.h:1040-1182) for unsigned and signed bm::sparse_vector<> and
+// bm::rsc_sparse_vector<>.
 //
 // The scanner binds to one sparse vector (like sparse_vector_scanner::bind, :1060): its bit-planes
 // (sparse_vector::get_slice(j), j < effective_slices()) and its searchable universe (the NOT-NULL plane of a nullable
@@ -14,6 +15,9 @@
 // [0, effective_size()) and the NOT-NULL vector NN, as wide as the logical space; the device rs index of NN is built once.
 // A search scans the compressed columns and bmb200_rank_decompress maps the result to logical positions, as the reference
 // scanner does for RSC vectors (src/bmsparsevec_algo.h:2300-2306,4525-4537); results are in the logical index space.
+// A signed vector (value_type int32_t / int64_t) stores s2u(x) in its planes (src/bmbmatrix.h:2536-2569, plane 0 = sign);
+// its searches run with BMB200_F_SIGNED and the value as a two's-complement int64_t.  find_zero / find_nonzero stay unsigned
+// EQ 0 / GT 0 over the same planes, which is what the reference computes for them (an OR of all planes).
 // bm::b200::rank_compressor<BV> is the device counterpart of bm::rank_compressor<BV> (src/bmalgo.h:451-644).
 #ifndef BMB200_SCANNER_HPP_INCLUDED
 #define BMB200_SCANNER_HPP_INCLUDED
@@ -31,7 +35,7 @@ public:
     typedef typename SV::bvector_type bvector_type;
     typedef typename SV::value_type value_type;
     typedef typename bvector_type::size_type size_type;
-    static_assert(!std::is_signed<value_type>::value, "bm::b200::scanner: unsigned sparse vectors only");
+    static constexpr bool is_signed = std::is_signed<value_type>::value;
 
     scanner(context& c, const SV& sv) : ctx_(c) { bind(sv); }
     ~scanner() { if (rs_) bmb200_rs_free(rs_); if (set_) bmb200_set_free(set_); }
@@ -76,34 +80,42 @@ public:
     void find_lt(value_type v, bvector_type& bv_out) { one(BMB200_SCAN_LT, v, 0, bv_out); }
     void find_le(value_type v, bvector_type& bv_out) { one(BMB200_SCAN_LE, v, 0, bv_out); }
     void find_range(value_type from, value_type to, bvector_type& bv_out) { one(BMB200_SCAN_RANGE, from, to, bv_out); }
-    void find_zero(bvector_type& bv_out)    { one(BMB200_SCAN_EQ, 0, 0, bv_out); }
-    void find_nonzero(bvector_type& bv_out) { one(BMB200_SCAN_GT, 0, 0, bv_out); }
+    // sign-agnostic in the reference (an OR of all planes): the unsigned search for 0 also on a signed vector
+    void find_zero(bvector_type& bv_out)    { const uint64_t z[2] = {0, 0}; run(BMB200_SCAN_EQ, z, 1, &bv_out, nullptr, false); }
+    void find_nonzero(bvector_type& bv_out) { const uint64_t z[2] = {0, 0}; run(BMB200_SCAN_GT, z, 1, &bv_out, nullptr, false); }
 
-    /// batched searches: one launch, out[k] replaced by the result of values[k]
+    /// batched searches: one launch, out[k] replaced by the result of values[k].  For a signed vector every slot holds
+    /// a two's-complement int64_t: uint64_t(int64_t(v)).
     void find_batch(int pred, const std::vector<uint64_t>& values, std::vector<bvector_type>& out)
     {
         const size_t nv = pred == BMB200_SCAN_RANGE ? values.size() / 2 : values.size();
         out.resize(nv);
-        run(pred, values.data(), (uint32_t)nv, out.data(), nullptr);
+        run(pred, values.data(), (uint32_t)nv, out.data(), nullptr, is_signed);
     }
-    /// cardinalities only (pipeline agg_opt_only_counts)
+    /// cardinalities only (pipeline agg_opt_only_counts); values as in find_batch
     void count_batch(int pred, const std::vector<uint64_t>& values, std::vector<size_type>& counts)
     {
         const size_t nv = pred == BMB200_SCAN_RANGE ? values.size() / 2 : values.size();
         counts.assign(nv, 0);
-        run(pred, values.data(), (uint32_t)nv, nullptr, counts.data());
+        run(pred, values.data(), (uint32_t)nv, nullptr, counts.data(), is_signed);
     }
 
 private:
+    static uint64_t slot(value_type v)
+    {
+        if constexpr (is_signed) return uint64_t(int64_t(v));
+        else return uint64_t(v);
+    }
     void one(int pred, value_type a, value_type b, bvector_type& bv_out)
     {
-        const uint64_t v[2] = {uint64_t(a), uint64_t(b)};
-        run(pred, v, 1, &bv_out, nullptr);
+        const uint64_t v[2] = {slot(a), slot(b)};
+        run(pred, v, 1, &bv_out, nullptr, is_signed);
     }
-    void run(int pred, const uint64_t* values, uint32_t nv, bvector_type* out, size_type* counts)
+    void run(int pred, const uint64_t* values, uint32_t nv, bvector_type* out, size_type* counts, bool sgn)
     {
         if (!nv) return;
-        bmb200_scan_args a{0u, n_planes_, n_planes_, pred, out ? BMB200_F_OPT_COMPRESS : BMB200_F_COUNT_ONLY, values, nv, 0u, scan_to_};
+        const uint32_t flags = (out ? BMB200_F_OPT_COMPRESS : BMB200_F_COUNT_ONLY) | (sgn ? BMB200_F_SIGNED : 0u);
+        bmb200_scan_args a{0u, n_planes_, n_planes_, pred, flags, values, nv, 0u, scan_to_};
         bmb200_result* res = nullptr;
         int rc = bmb200_scan(ctx_.get(), set_, &a, &res);
         if constexpr (SV::is_compressed()) {

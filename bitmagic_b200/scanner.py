@@ -12,29 +12,42 @@ this module only packs planes and calls the C ABI (``bmb200_scan``).
 A rank-select compressed vector (``bm::rsc_sparse_vector<unsigned>``, src/bmsparsevec_compr.h) is searched the way the
 reference searches it (src/bmsparsevec_algo.h:2300-2306,4525-4537): the scan runs over its compressed planes, restricted to
 ``[0, effective_size())``, and ``bmb200_rank_decompress`` maps the result to logical positions through the NOT-NULL vector.
+
+Signed vectors (``sparse_vector<int32_t / int64_t>`` and their RSC forms; ``from_values(..., signed=True)``) store every
+element as ``s2u(x)`` (src/bmbmatrix.h:2536-2569: ``x >= 0 -> x << 1``, ``x < 0 -> (-(x+1)) << 1 | 1``), so plane 0 is the
+sign plane.  Their searches take int64 values and run with ``F_SIGNED``; ``find_zero / find_nonzero`` stay unsigned searches
+for 0 over the same planes, which is what the reference computes for them (an OR of all planes).
 """
 from __future__ import annotations
 
 import numpy as np
 
 from . import capi
-from .capi import F_COUNT_ONLY, F_OPT_COMPRESS, SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT, SCAN_RANGE
+from .capi import F_COUNT_ONLY, F_OPT_COMPRESS, F_SIGNED, SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT, SCAN_RANGE
 from .hostfmt import BLOCK_BITS, BVector, PackedSet, bits_to_words, result_to_bvector
+
+
+def s2u(values) -> np.ndarray:
+    """sparse_vector<signed>::s2u (src/bmbmatrix.h:2536-2569) of int64 values: x >= 0 -> x << 1, x < 0 -> (-(x+1)) << 1 | 1."""
+    x = np.ascontiguousarray(values, dtype=np.int64)
+    return np.where(x >= 0, x.view(np.uint64) << np.uint64(1), ((~x).view(np.uint64) << np.uint64(1)) | np.uint64(1))
 
 
 class SparseVector:
     """``bm::sparse_vector<unsigned, bvector<>>`` as the scanner sees it: ``size()``, ``effective_slices()`` planes and,
     for a nullable vector, the NOT-NULL plane (``get_null_bvector()``)."""
 
-    def __init__(self, planes: list[BVector], size: int, not_null: BVector | None = None):
+    def __init__(self, planes: list[BVector], size: int, not_null: BVector | None = None, signed: bool = False):
         self.planes = planes
         self.size = int(size)
         self.not_null = not_null
+        self.signed = bool(signed)
 
     @classmethod
-    def from_values(cls, values, null_mask=None, optimize: bool = True) -> "SparseVector":
-        """import(values) [+ set_null where null_mask] + optimize(): plane j = elements with bit j set."""
-        v = np.ascontiguousarray(values, dtype=np.uint64)
+    def from_values(cls, values, null_mask=None, optimize: bool = True, signed: bool = False) -> "SparseVector":
+        """import(values) [+ set_null where null_mask] + optimize(): plane j = elements with bit j set.  signed: the values are
+        int64 and the planes hold s2u(value) (plane 0 = sign), as in sparse_vector<int32_t / int64_t>."""
+        v = s2u(values) if signed else np.ascontiguousarray(values, dtype=np.uint64)
         n = v.size
         nb = max(1, (n + BLOCK_BITS - 1) // BLOCK_BITS)
         if null_mask is not None:
@@ -53,7 +66,7 @@ class SparseVector:
             nn = BVector.from_words(bits_to_words(bits))
             if optimize:
                 nn.optimize()
-        return cls(planes, n, nn)
+        return cls(planes, n, nn, signed)
 
     def effective_slices(self) -> int:
         return len(self.planes)
@@ -73,23 +86,25 @@ class RscSparseVector:
     positions ``[0, effective_size())`` in index order; ``not_null`` (``get_null_bvector()``) maps them back to the logical
     index space of ``size`` positions."""
 
-    def __init__(self, planes: list[BVector], size: int, not_null: BVector):
+    def __init__(self, planes: list[BVector], size: int, not_null: BVector, signed: bool = False):
         self.planes = planes
         self.size = int(size)
         self.not_null = not_null
+        self.signed = bool(signed)
         self._eff = not_null.count()
 
     @classmethod
-    def from_values(cls, values, null_mask, optimize: bool = True) -> "RscSparseVector":
-        """The nullable sparse vector of from_values(values, null_mask), rank-compressed (rsc_sparse_vector::load_from)."""
-        v = np.ascontiguousarray(values, dtype=np.uint64)
+    def from_values(cls, values, null_mask, optimize: bool = True, signed: bool = False) -> "RscSparseVector":
+        """The nullable sparse vector of from_values(values, null_mask), rank-compressed (rsc_sparse_vector::load_from).
+        signed: int64 values, s2u planes (rsc_sparse_vector<int32_t / int64_t>)."""
+        v = np.ascontiguousarray(values, dtype=np.int64 if signed else np.uint64)
         keep = ~np.asarray(null_mask, bool)
-        dense = SparseVector.from_values(v[keep], None, optimize)
+        dense = SparseVector.from_values(v[keep], None, optimize, signed)
         nb = max(1, (v.size + BLOCK_BITS - 1) // BLOCK_BITS)
         bits = np.zeros(nb * BLOCK_BITS, np.uint8)
         bits[:v.size] = keep
         nn = BVector.from_words(bits_to_words(bits))
-        return cls(dense.planes, v.size, nn.optimize() if optimize else nn)
+        return cls(dense.planes, v.size, nn.optimize() if optimize else nn, signed)
 
     def effective_size(self) -> int:
         return self._eff
@@ -134,10 +149,13 @@ class SparseVectorScanner:
             self._dset.free()
             self._dset = None
 
-    def _run(self, pred, values, count_only=False):
+    def _run(self, pred, values, count_only=False, signed=None):
+        """signed: compare as signed values (default: the vector's signedness); find_zero / find_nonzero pass False"""
+        signed = self.sv.signed if signed is None else signed
         single = np.ndim(values) == (1 if pred == SCAN_RANGE else 0)
-        vals = np.atleast_2d(values) if pred == SCAN_RANGE else np.atleast_1d(values)
-        flags = F_COUNT_ONLY if count_only else F_OPT_COMPRESS
+        dt = np.int64 if signed else np.uint64
+        vals = np.atleast_2d(np.asarray(values, dt)) if pred == SCAN_RANGE else np.atleast_1d(np.asarray(values, dt))
+        flags = (F_COUNT_ONLY if count_only else F_OPT_COMPRESS) | (F_SIGNED if signed else 0)
         res = capi.scan(self.ctx, self._dset, pred, vals, 0, self.sv.effective_slices(), self._universe, flags, 0, self._scan_to)
         try:
             nv = vals.shape[0]
@@ -164,10 +182,11 @@ class SparseVectorScanner:
     def find_lt(self, value):    return self._run(SCAN_LT, value)
     def find_le(self, value):    return self._run(SCAN_LE, value)
     def find_range(self, lo, hi=None):
-        return self._run(SCAN_RANGE, np.array([lo, hi], np.uint64) if hi is not None else lo)
-    def find_zero(self):         return self._run(SCAN_EQ, 0)
-    def find_nonzero(self):      return self._run(SCAN_GT, 0)
+        return self._run(SCAN_RANGE, [lo, hi] if hi is not None else lo)
+    # sign-agnostic (the reference ORs every plane, sign included): unsigned EQ 0 / GT 0 also for a signed vector
+    def find_zero(self):         return self._run(SCAN_EQ, 0, signed=False)
+    def find_nonzero(self):      return self._run(SCAN_GT, 0, signed=False)
     def count_eq(self, value):   return self._run(SCAN_EQ, value, True)
     def count_gt(self, value):   return self._run(SCAN_GT, value, True)
     def count_range(self, lo, hi=None):
-        return self._run(SCAN_RANGE, np.array([lo, hi], np.uint64) if hi is not None else lo, True)
+        return self._run(SCAN_RANGE, [lo, hi] if hi is not None else lo, True)

@@ -90,6 +90,8 @@ extern "C" {
 #define BMB200_F_OPT_NONE    0u  /* result kinds as aggregator opt_mode_ == opt_none           */
 #define BMB200_F_OPT_COMPRESS 2u /* classify + bit->GAP like opt_copy_bit_block(opt_compress) */
 #define BMB200_F_OR_TARGET   4u  /* batch only: also accumulate the union of all group results (pipeline::set_or_target) */
+#define BMB200_F_SIGNED      8u  /* bmb200_scan only: the planes hold s2u-encoded signed elements (plane plane0 = sign plane)
+                                  * and values[] are int64_t in two's complement (see bmb200_scan)                         */
 
 typedef struct bmb200_ctx    bmb200_ctx;     /* one per process per GPU                      */
 typedef struct bmb200_set    bmb200_set;     /* device-resident column-major set of vectors  */
@@ -330,7 +332,12 @@ int bmb200_result_free(bmb200_result* res);
 /* sparse_vector_scanner<SV> searches over the bit-planes ("slices", bm::sparse_vector::get_slice(i),
  * src/bmsparsevec.h) of ONE unsigned sparse vector stored as vectors of a set: plane j (bit j of every element) is set
  * vector plane0 + j.  One launch answers n_values searches; the result has n_values * n_cols columns, value-major,
- * exactly like a pipeline batch (per-value cardinalities through bmb200_result_group_totals). */
+ * exactly like a pipeline batch (per-value cardinalities through bmb200_result_group_totals).
+ * Signed vectors (bm::sparse_vector<int32_t / int64_t>, rsc_sparse_vector<int32_t / int64_t>) are searched with
+ * BMB200_F_SIGNED: element x is stored as u = s2u(x) (src/bmbmatrix.h: x >= 0 -> x << 1, x < 0 -> (-(x+1)) << 1 | 1), so
+ * plane0 is the sign plane and planes 1..n_planes-1 hold the magnitude; values[] are then int64_t (passed in the uint64_t
+ * slots), compared as signed integers, and RANGE swaps reversed bounds by signed order.  find_zero / find_nonzero of a
+ * signed vector are the unsigned EQ 0 / GT 0 over the same planes (the reference ORs all planes, sign included). */
 #define BMB200_SCAN_EQ     0   /* find_eq    src/bmsparsevec_algo.h:1083  elements == value                    */
 #define BMB200_SCAN_GT     1   /* find_gt    :1135                        elements >  value                    */
 #define BMB200_SCAN_GE     2   /* find_ge    :1144                                                             */
@@ -344,8 +351,9 @@ typedef struct bmb200_scan_args {
                                  * the NOT-NULL plane for a nullable one (what finalize_search_result and
                                  * invert_internal apply, :2426,1686); 0xffffffff = every index of the columns */
     int32_t         pred;       /* BMB200_SCAN_*                                                              */
-    uint32_t        flags;      /* BMB200_F_COUNT_ONLY / BMB200_F_OPT_COMPRESS                                */
-    const uint64_t* values;     /* HOST: n_values search values (RANGE: 2 * n_values, lo then hi)             */
+    uint32_t        flags;      /* BMB200_F_COUNT_ONLY / BMB200_F_OPT_COMPRESS, | BMB200_F_SIGNED              */
+    const uint64_t* values;     /* HOST: n_values search values (RANGE: 2 * n_values, lo then hi);
+                                 * with BMB200_F_SIGNED each is an int64_t in two's complement                */
     uint32_t        n_values;
     uint32_t        nb_from;
     uint32_t        nb_to;      /* 0 == n_blocks */
