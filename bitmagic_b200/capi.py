@@ -24,6 +24,8 @@ BLK_NULL, BLK_FULL, BLK_BIT, BLK_GAP = 0, 1, 2, 3
 OP_OR, OP_AND, OP_AND_SUB, OP_XOR, OP_SHIFT_R_AND = 0, 1, 2, 3, 4
 F_COUNT_ONLY, F_OPT_NONE, F_OPT_COMPRESS, F_OR_TARGET = 1, 0, 2, 4
 F_SIGNED = 8                  # bmb200_scan: s2u planes (plane0 = sign plane), int64 search values
+F_STR_PREFIX = 16             # bmb200_scan_str: compare the first strlen(s) bytes (find_eq_str_prefix)
+STR_MAX_PLANES = 2048         # bmb200_scan_str: n_planes limit (strings of up to 256 bytes)
 
 # every symbol include/bmb200.h declares (checked by tests/test_cabi_symbols.py)
 SYMBOLS = [
@@ -42,7 +44,7 @@ SYMBOLS = [
     "bmb200_set_upload_slabs", "bmb200_host_slabs_prefetch", "bmb200_host_slab_alloc", "bmb200_host_slab_free",
     "bmb200_result_fetch_view_async", "bmb200_result_fetch_wait", "bmb200_exchange_mode",
     "bmb200_result_fetch_column", "bmb200_set_run_lists", "bmb200_set_bit_run_lists",
-    "bmb200_rank_decompress", "bmb200_rank_compress",
+    "bmb200_rank_decompress", "bmb200_rank_compress", "bmb200_scan_str",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
@@ -91,6 +93,14 @@ class ScanArgsC(C.Structure):
         ("plane0", C.c_uint32), ("n_planes", C.c_uint32), ("universe", C.c_uint32),
         ("pred", C.c_int32), ("flags", C.c_uint32),
         ("values", C.c_void_p), ("n_values", C.c_uint32),
+        ("nb_from", C.c_uint32), ("nb_to", C.c_uint32),
+    ]
+
+
+class ScanStrArgsC(C.Structure):
+    _fields_ = [
+        ("plane0", C.c_uint32), ("n_planes", C.c_uint32), ("universe", C.c_uint32), ("flags", C.c_uint32),
+        ("strs", C.c_void_p), ("stride", C.c_uint32), ("n_values", C.c_uint32),
         ("nb_from", C.c_uint32), ("nb_to", C.c_uint32),
     ]
 
@@ -558,6 +568,35 @@ def scan(ctx: Context, dset: DeviceSet, pred: int, values, plane0: int, n_planes
     args = ScanArgsC(int(plane0), int(n_planes), int(universe), int(pred), int(flags), ptr(vals), int(nv), int(nb_from), int(nb_to))
     res = result if result is not None else DeviceResult(ctx)
     ctx.check(lib().bmb200_scan(ctx._h, dset._h, C.byref(args), C.byref(res._h)), "scan")
+    res.n_cols = ((nb_to if nb_to else dset.n_blocks) - nb_from) * int(nv)
+    return res
+
+
+def str_slots(strs) -> tuple[np.ndarray, int]:
+    """byte strings -> (n, stride) uint8 array of NUL-padded slots (stride = longest + 1)"""
+    bs = [bytes(x) for x in strs]
+    stride = max(len(b) for b in bs) + 1 if bs else 1
+    a = np.zeros((len(bs), stride), np.uint8)
+    for k, b in enumerate(bs):
+        a[k, :len(b)] = np.frombuffer(b, np.uint8)
+    return a, stride
+
+
+def scan_str(ctx: Context, dset: DeviceSet, strs, plane0: int, n_planes: int, universe: int = NO_UNIVERSE, flags: int = 0,
+             nb_from: int = 0, nb_to: int = 0, result: DeviceResult | None = None) -> DeviceResult:
+    """bmb200_scan_str: string equality (F_STR_PREFIX: prefix) of the string sparse vector whose plane 8k+b is set vector
+    plane0 + 8k + b against every query (a list of bytes, or an (n, stride) uint8 array of NUL-padded slots); the result has
+    n_values * n_cols columns, value-major."""
+    if isinstance(strs, np.ndarray):
+        slots = np.ascontiguousarray(strs, dtype=np.uint8)
+        stride = slots.shape[1]
+    else:
+        slots, stride = str_slots(strs)
+    nv = slots.shape[0]
+    args = ScanStrArgsC(int(plane0), int(n_planes), int(universe), int(flags), ptr(slots) if slots.size else C.c_void_p(0),
+                        int(stride), int(nv), int(nb_from), int(nb_to))
+    res = result if result is not None else DeviceResult(ctx)
+    ctx.check(lib().bmb200_scan_str(ctx._h, dset._h, C.byref(args), C.byref(res._h)), "scan_str")
     res.n_cols = ((nb_to if nb_to else dset.n_blocks) - nb_from) * int(nv)
     return res
 

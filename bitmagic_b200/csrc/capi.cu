@@ -12,6 +12,7 @@
 #include "aux_kernels.cuh"
 #include "runlist_kernel.cuh"
 #include "scan_kernel.cuh"
+#include "str_scan_kernel.cuh"
 #include "rank_kernel.cuh"
 #include "shift_kernel.cuh"
 #include "binop_kernel.cuh"
@@ -1606,6 +1607,85 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
     else if (mode == 1) { if (vg == 2) BMB200_SCAN_LAUNCH(2, 1); else BMB200_SCAN_LAUNCH(1, 1); }
     else                { if (vg == 2) BMB200_SCAN_LAUNCH(2, 2); else BMB200_SCAN_LAUNCH(1, 2); }
     #undef BMB200_SCAN_LAUNCH
+    if ((rc = after_launch(ctx))) return bail(rc);
+    *inout = r;
+    if (store && compress) r->gaps_ready = true;
+    return BMB200_OK;
+}
+
+int bmb200_scan_str(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_str_args* a, bmb200_result** inout)
+{
+    if (!ctx || !set || !a || !inout || set->ctx != ctx || !a->strs || !a->stride || !a->n_values) return BMB200_ERR_BADARG;
+    if (!a->n_planes || a->n_planes > kStrMaxPlanes) return BMB200_ERR_BADARG;
+    if (a->flags & ~(BMB200_F_COUNT_ONLY | BMB200_F_OPT_COMPRESS | BMB200_F_STR_PREFIX)) return BMB200_ERR_BADARG;
+    if ((uint64_t)a->plane0 + a->n_planes > set->v.n_vec) return BMB200_ERR_RANGE;
+    if (a->universe != 0xffffffffu && a->universe >= set->v.n_vec) return BMB200_ERR_RANGE;
+    const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
+    if (a->nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
+    const uint32_t cols = nb_to - a->nb_from, nv = a->n_values;
+    const uint64_t tot_cols = (uint64_t)cols * nv;
+    if (tot_cols > 0x7fffffffull) return BMB200_ERR_RANGE;
+
+    // every query -> its limit word + its bytes as plane bits (little-endian words: plane j = bit j & 31 of word j >> 5)
+    const bool prefix = (a->flags & BMB200_F_STR_PREFIX) != 0;
+    const uint32_t n_planes = a->n_planes, vw = 1u + (n_planes + 31u) / 32u, n_bytes = (n_planes + 7u) / 8u;
+    std::vector<uint32_t> staged;
+    try { staged.assign((size_t)nv * vw, 0u); } catch (...) { return BMB200_ERR_BADALLOC; }
+    for (uint32_t k = 0; k < nv; ++k) {
+        const unsigned char* s = reinterpret_cast<const unsigned char*>(a->strs) + (size_t)k * a->stride;
+        const void* nul = memchr(s, 0, a->stride);
+        if (!nul) return BMB200_ERR_BADARG;                 // no terminator inside the slot
+        const uint32_t len = (uint32_t)(static_cast<const unsigned char*>(nul) - s);
+        uint32_t* w = staged.data() + (size_t)k * vw;
+        bool dead = false;
+        for (uint32_t i = 0; i < len; ++i) {
+            uint32_t c = s[i];
+            if (8u * i + 8u > n_planes) {                   // bits of this byte at planes >= n_planes: no element has them
+                const uint32_t keep = 8u * i >= n_planes ? 0u : n_planes - 8u * i;
+                if (c >> keep) { dead = true; break; }
+            }
+            if (i < n_bytes) w[1 + i / 4] |= c << (8u * (i & 3u));
+        }
+        // the empty string is the exact search for all-zero elements in either mode (find_zero, :3412-3416)
+        const uint32_t lim = (prefix && len) ? std::min(8u * len, n_planes) : n_planes;
+        w[0] = dead ? kStrDead : lim;
+    }
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t n_cols = (uint32_t)tot_cols;
+    const bool store = !(a->flags & BMB200_F_COUNT_ONLY);
+    const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
+
+    bmb200_result* r = *inout;
+    if (r && (r->ctx != ctx || r->n_cols != n_cols || r->n_groups != nv || (store && !r->blocks) ||
+              (store && compress && !r->gaps) || r->or_blocks)) {
+        bmb200_result_free(r); r = nullptr; *inout = nullptr;
+    }
+    if (!r) {
+        int rc = result_alloc(ctx, n_cols, nv, store, store && compress, false, &r);
+        if (rc) return rc;
+    }
+    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
+    r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
+
+    int rc = stage_group(ctx, staged.data(), staged.size(), nullptr, 0, false);
+    if (rc) return bail(rc);
+    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8 * (size_t)nv, ctx->stream);
+    if (e != cudaSuccess) { ctx->last_err = std::string("scan_str: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
+
+    StrScanParams sp{};
+    sp.out = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
+    sp.out.n_groups = nv;
+    sp.plane0 = a->plane0; sp.n_planes = n_planes; sp.universe = a->universe; sp.vwords = vw;
+    sp.strs = ctx->d_group;
+    // queries per pass as for find_eq: 4 when the batch has them, single searches on the narrow kernel
+    const uint32_t vg = nv == 1 ? 1u : nv >= 4 ? 4u : 2u;
+    const uint64_t items = (uint64_t)cols * ((nv + vg - 1) / vg);
+    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
+    if (grid > items) grid = (uint32_t)items;
+    if (vg == 4) str_scan_kernel<4><<<grid, kAggThreads, 0, ctx->stream>>>(sp);
+    else if (vg == 2) str_scan_kernel<2><<<grid, kAggThreads, 0, ctx->stream>>>(sp);
+    else str_scan_kernel<1><<<grid, kAggThreads, 0, ctx->stream>>>(sp);
     if ((rc = after_launch(ctx))) return bail(rc);
     *inout = r;
     if (store && compress) r->gaps_ready = true;

@@ -232,6 +232,37 @@ struct set_uploader
         return bmb200_set_upload_vectors(ctx, n_vec, n_blocks, vb, set);
     }
 };
+
+/// Lowest set bit in [b0, b1] of result column `col` (one column read back: bmb200_result_fetch_column); 65536 when there is
+/// none.  What aggregator::find_first_and_sub reads once the popcounts have located a non-empty column (src/bmaggregator.h:1538-1546).
+inline unsigned result_column_first(bmb200_result* res, uint32_t col, unsigned b0 = 0u, unsigned b1 = 65535u)
+{
+    uint8_t kd = 0; std::vector<uint32_t> bits(BMB200_BLOCK_WORDS); std::vector<uint16_t> gaps(BMB200_GAP_MAX_WORDS);
+    check(bmb200_result_fetch_column(res, col, &kd, bits.data(), gaps.data()), "bmb200_result_fetch_column");
+    unsigned first = 65536u;
+    if (kd == BMB200_BLK_FULL) first = b0;
+    else if (kd == BMB200_BLK_BIT)
+    {
+        for (unsigned w = b0 >> 5; w <= (b1 >> 5) && first == 65536u; ++w)
+        {
+            uint32_t x = bits[w];
+            if (w == (b0 >> 5)) x &= ~0u << (b0 & 31u);
+            if (w == (b1 >> 5) && (b1 & 31u) != 31u) x &= (1u << ((b1 & 31u) + 1u)) - 1u;
+            if (x) first = (w << 5) + (unsigned)__builtin_ctz(x);
+        }
+    }
+    else if (kd == BMB200_BLK_GAP)
+    {
+        const unsigned len = gaps[0] >> 3; unsigned val = gaps[0] & 1u, start = 0;
+        for (unsigned k = 1; k <= len && first == 65536u; ++k, val ^= 1u)
+        {
+            const unsigned end = gaps[k];
+            if (val && end >= b0 && start <= b1) first = std::max(start, b0);
+            start = end + 1u;
+        }
+    }
+    return first;
+}
 }  // namespace detail
 
 /// Residency: a set of bvectors uploaded ONCE (block trees walked and blocks packed by host threads, H2D pipelined -- all inside
@@ -398,32 +429,9 @@ public:
             for (uint32_t nb = std::max(sp.first, lo); nb < std::min(sp.second, hi); ++nb)
             {
                 if (!pop[nb - lo]) continue;
-                uint8_t kd = 0; std::vector<uint32_t> bits(BMB200_BLOCK_WORDS); std::vector<uint16_t> gaps(BMB200_GAP_MAX_WORDS);
-                check(bmb200_result_fetch_column(res, nb - lo, &kd, bits.data(), gaps.data()), "bmb200_result_fetch_column");
                 unsigned b0 = one_block ? (unsigned)(range_from_ & bm::set_block_mask) : 0u,
                          b1 = one_block ? (unsigned)(range_to_ & bm::set_block_mask) : 65535u;
-                unsigned first = 65536u;
-                if (kd == BMB200_BLK_FULL) first = b0;
-                else if (kd == BMB200_BLK_BIT)
-                {
-                    for (unsigned w = b0 >> 5; w <= (b1 >> 5) && first == 65536u; ++w)
-                    {
-                        uint32_t x = bits[w];
-                        if (w == (b0 >> 5)) x &= ~0u << (b0 & 31u);
-                        if (w == (b1 >> 5) && (b1 & 31u) != 31u) x &= (1u << ((b1 & 31u) + 1u)) - 1u;
-                        if (x) first = (w << 5) + (unsigned)__builtin_ctz(x);
-                    }
-                }
-                else if (kd == BMB200_BLK_GAP)
-                {
-                    const unsigned len = gaps[0] >> 3; unsigned val = gaps[0] & 1u, start = 0;
-                    for (unsigned k = 1; k <= len && first == 65536u; ++k, val ^= 1u)
-                    {
-                        const unsigned end = gaps[k];
-                        if (val && end >= b0 && start <= b1) first = std::max(start, b0);
-                        start = end + 1u;
-                    }
-                }
+                const unsigned first = detail::result_column_first(res, nb - lo, b0, b1);
                 if (first != 65536u) { idx = (size_type)((uint64_t)nb * 65536u + first); return true; }
                 if (one_block) return false;
             }

@@ -18,6 +18,10 @@
 // A signed vector (value_type int32_t / int64_t) stores s2u(x) in its planes (src/bmbmatrix.h:2536-2569, plane 0 = sign);
 // its searches run with BMB200_F_SIGNED and the value as a two's-complement int64_t.  find_zero / find_nonzero stay unsigned
 // EQ 0 / GT 0 over the same planes, which is what the reference computes for them (an OR of all planes).
+// A string vector (bm::str_sparse_vector<char, ...>, SV::is_str()) binds its planes j < rows_not_null() (plane 8k+b = bit b of
+// byte k) and its universe; find_eq_str / find_eq_str_prefix / the batched string searches are bmb200_scan_str launches
+// (csrc/str_scan_kernel.cuh).  A remapped vector's queries are translated on the host (remap_tosv) and only their codes go to
+// the device.  The numeric searches do not compile for a string vector.
 // bm::b200::rank_compressor<BV> is the device counterpart of bm::rank_compressor<BV> (src/bmalgo.h:451-644).
 #ifndef BMB200_SCANNER_HPP_INCLUDED
 #define BMB200_SCANNER_HPP_INCLUDED
@@ -25,6 +29,8 @@
 #include "bmsparsevec.h"
 #include "bmsparsevec_algo.h"
 #include "bmb200_aggregator.hpp"
+
+#include <string>
 
 namespace bm { namespace b200 {
 
@@ -47,8 +53,16 @@ public:
         if (rs_) { bmb200_rs_free(rs_); rs_ = nullptr; }
         if (set_) { bmb200_set_free(set_); set_ = nullptr; }
         size_ = sv.size();
-        n_planes_ = sv.effective_slices();
-        while (n_planes_ > 1 && !sv.get_slice(n_planes_ - 1)) --n_planes_;
+        if constexpr (SV::is_str()) {
+            // rows_not_null() string planes, trailing absent ones trimmed (their bits are all 0)
+            str_sv_ = &sv;
+            n_planes_ = (unsigned)sv.get_bmatrix().rows_not_null();
+            while (n_planes_ > 1 && !sv.get_slice(n_planes_ - 1)) --n_planes_;
+            if (!n_planes_) n_planes_ = 1;
+        } else {
+            n_planes_ = sv.effective_slices();
+            while (n_planes_ > 1 && !sv.get_slice(n_planes_ - 1)) --n_planes_;
+        }
         n_blocks_ = (uint32_t)((uint64_t(size_) + 65535ull) >> 16); if (!n_blocks_) n_blocks_ = 1;
         const bvector_type* nn = sv.get_null_bvector();
         uint32_t n_vec = n_planes_ + 1;
@@ -66,7 +80,7 @@ public:
         std::vector<bmb200_vec_blocks> vb(n_vec);
         bvector_type empty;
         for (unsigned j = 0; j < n_vec; ++j) {
-            const bvector_type* bv = j < n_planes_ ? sv.get_slice(j) : j == n_planes_ ? &universe_ : nn;
+            const bvector_type* bv = j < n_planes_ ? plane(sv, j) : j == n_planes_ ? &universe_ : nn;
             views[j].build(bv ? *bv : empty, n_blocks_);                 // planes past their columns stay NULL
             vb[j].n_blocks = n_blocks_; vb[j].kind = views[j].kind.data(); vb[j].ptr = views[j].ptr.data();
         }
@@ -83,6 +97,44 @@ public:
     // sign-agnostic in the reference (an OR of all planes): the unsigned search for 0 also on a signed vector
     void find_zero(bvector_type& bv_out)    { const uint64_t z[2] = {0, 0}; run(BMB200_SCAN_EQ, z, 1, &bv_out, nullptr, false); }
     void find_nonzero(bvector_type& bv_out) { const uint64_t z[2] = {0, 0}; run(BMB200_SCAN_GT, z, 1, &bv_out, nullptr, false); }
+
+    // ---- string vectors (str_sparse_vector): find_eq_str / find_eq_str_prefix, src/bmsparsevec_algo.h:3263-3436 ----
+    /// elements equal to s; false when there is none (or the vector is empty)
+    bool find_eq_str(const char* s, bvector_type& bv_out) { str_run(&s, 1, 0u, &bv_out, nullptr); return bv_out.any(); }
+    /// elements whose first strlen(s) bytes are s (the empty s: find_eq_str(""))
+    bool find_eq_str_prefix(const char* s, bvector_type& bv_out) { str_run(&s, 1, BMB200_F_STR_PREFIX, &bv_out, nullptr); return bv_out.any(); }
+    /// the lowest element equal to s (find_first_eq): one launch, the first non-empty column read back
+    bool find_eq_str(const char* s, size_type& pos)
+    {
+        static_assert(SV::is_str(), "find_eq_str needs a str_sparse_vector");
+        std::vector<std::string> codes;
+        if (!size_ || !to_codes(&s, 1, codes)) return false;
+        bmb200_result* res = launch_str(codes, BMB200_F_OPT_NONE);
+        struct drop { bmb200_result* r; ~drop() { bmb200_result_free(r); } } guard{res};
+        std::vector<uint32_t> pop(n_blocks_);
+        bmb200_result_meta m{}; m.popcnt = pop.data();
+        check(bmb200_result_fetch_meta(res, &m), "bmb200_result_fetch_meta");
+        for (uint32_t nb = 0; nb < n_blocks_; ++nb) {
+            if (!pop[nb]) continue;
+            const unsigned first = detail::result_column_first(res, nb);
+            if (first != 65536u) { pos = (size_type)((uint64_t)nb * 65536u + first); return true; }
+        }
+        return false;
+    }
+    /// pipeline + find_eq_str(TPipe&) (src/bmsparsevec_algo.h:3424-3436,4579-4651): one launch, out[k] = exact result of q[k]
+    void find_eq_str_batch(const std::vector<std::string>& q, std::vector<bvector_type>& out)
+    {
+        std::vector<const char*> p(q.size()); for (size_t k = 0; k < q.size(); ++k) p[k] = q[k].c_str();
+        out.resize(q.size());
+        str_run(p.data(), p.size(), 0u, out.data(), nullptr);
+    }
+    /// the same searches, cardinalities only (pipeline<agg_opt_only_counts>)
+    void count_eq_str_batch(const std::vector<std::string>& q, std::vector<size_type>& counts)
+    {
+        std::vector<const char*> p(q.size()); for (size_t k = 0; k < q.size(); ++k) p[k] = q[k].c_str();
+        counts.assign(q.size(), 0);
+        str_run(p.data(), p.size(), 0u, nullptr, counts.data());
+    }
 
     /// batched searches: one launch, out[k] replaced by the result of values[k].  For a signed vector every slot holds
     /// a two's-complement int64_t: uint64_t(int64_t(v)).
@@ -101,6 +153,74 @@ public:
     }
 
 private:
+    static const bvector_type* plane(const SV& sv, unsigned j)
+    {
+        if constexpr (SV::is_str()) return j < sv.get_bmatrix().rows_not_null() ? sv.get_slice(j) : nullptr;
+        else return sv.get_slice(j);
+    }
+    /// the device form of each query: a remapped vector's codes (remap_tosv), else the bytes as they are.  Queries that cannot
+    /// match get ok = false: remap_tosv finds no code, or the reference has no defined answer for them (longer than
+    /// effective_max_str(), or a byte >= 0x80, whose remap row index sign-extends: DESIGN.md §3.5c).  -> any query left
+    bool to_codes(const char* const* q, size_t n, std::vector<std::string>& codes, std::vector<bool>* ok = nullptr)
+    {
+        codes.assign(n, std::string());
+        if (ok) ok->assign(n, false);
+        bool any = false;
+        for (size_t k = 0; k < n; ++k) {
+            const char* s = q[k];
+            bool good = true;
+            if (*s && str_sv_->is_remap()) {
+                const size_t len = std::strlen(s), ms = str_sv_->effective_max_str();
+                good = len <= ms;
+                for (size_t i = 0; good && i < len; ++i) good = (unsigned char)s[i] < 0x80u;
+                std::vector<char> buf(ms + 1, 0);
+                good = good && str_sv_->remap_tosv(buf.data(), ms, s);
+                if (good) codes[k] = buf.data();
+            } else codes[k] = s;
+            if (ok) (*ok)[k] = good;
+            any |= good;
+        }
+        return any;
+    }
+    /// one bmb200_scan_str launch over `codes` (NUL-padded slots of the longest + 1 bytes)
+    bmb200_result* launch_str(const std::vector<std::string>& codes, uint32_t flags)
+    {
+        size_t stride = 1;
+        for (const auto& c : codes) stride = std::max(stride, c.size() + 1);
+        std::vector<char> slots(codes.size() * stride, 0);
+        for (size_t k = 0; k < codes.size(); ++k) std::memcpy(slots.data() + k * stride, codes[k].data(), codes[k].size());
+        bmb200_scan_str_args a{0u, n_planes_, n_planes_, flags, slots.data(), (uint32_t)stride, (uint32_t)codes.size(), 0u, 0u};
+        bmb200_result* res = nullptr;
+        check(bmb200_scan_str(ctx_.get(), set_, &a, &res), "bmb200_scan_str");
+        return res;
+    }
+    /// string searches: out[k] / counts[k] of q[k]; a query that cannot match stays out of the launch and gets an empty slot
+    void str_run(const char* const* q, size_t n, uint32_t mode, bvector_type* out, size_type* counts)
+    {
+        static_assert(SV::is_str(), "string searches need a str_sparse_vector");
+        for (size_t k = 0; k < n; ++k) { if (out) out[k].clear(true); if (counts) counts[k] = 0; }
+        std::vector<std::string> codes; std::vector<bool> ok;
+        if (!n || !size_ || !to_codes(q, n, codes, &ok)) return;
+        std::vector<std::string> live; std::vector<size_t> at;
+        for (size_t k = 0; k < n; ++k) if (ok[k]) { live.push_back(codes[k]); at.push_back(k); }
+        bmb200_result* res = launch_str(live, mode | (out ? BMB200_F_OPT_COMPRESS : BMB200_F_COUNT_ONLY));
+        const uint32_t nv = (uint32_t)live.size();
+        const size_t ncols = (size_t)nv * n_blocks_;
+        std::vector<uint64_t> totals(nv);
+        std::vector<uint8_t> kind(ncols); std::vector<uint64_t> off(ncols); std::vector<uint32_t> bits; std::vector<uint16_t> gaps;
+        int rc = bmb200_result_group_totals(res, totals.data(), nv);
+        if (!rc && out) { uint64_t nb = 0, ng = 0; rc = bmb200_result_sizes(res, &nb, &ng);
+                          if (!rc) { bits.resize(nb * BMB200_BLOCK_WORDS); gaps.resize(ng);
+                                     rc = bmb200_result_fetch(res, kind.data(), off.data(), bits.data(), gaps.data()); } }
+        bmb200_result_free(res);
+        check(rc, "bmb200_scan_str");
+        for (uint32_t k = 0; k < nv; ++k) {
+            if (counts) counts[at[k]] = (size_type)totals[k];
+            if (out) detail::store_result(out[at[k]], size_, n_blocks_, kind.data() + (size_t)k * n_blocks_, off.data() + (size_t)k * n_blocks_,
+                                          bits.data(), gaps.data());
+        }
+    }
+
     static uint64_t slot(value_type v)
     {
         if constexpr (is_signed) return uint64_t(int64_t(v));
@@ -113,6 +233,7 @@ private:
     }
     void run(int pred, const uint64_t* values, uint32_t nv, bvector_type* out, size_type* counts, bool sgn)
     {
+        static_assert(!SV::is_str(), "a str_sparse_vector is searched with find_eq_str / find_eq_str_prefix");
         if (!nv) return;
         const uint32_t flags = (out ? BMB200_F_OPT_COMPRESS : BMB200_F_COUNT_ONLY) | (sgn ? BMB200_F_SIGNED : 0u);
         bmb200_scan_args a{0u, n_planes_, n_planes_, pred, flags, values, nv, 0u, scan_to_};
@@ -145,6 +266,7 @@ private:
     context& ctx_;
     bmb200_set* set_ = nullptr;
     bmb200_rs* rs_ = nullptr;          // RSC: rs index of NN
+    const SV* str_sv_ = nullptr;       // string vector: its remap tables stay on the host (to_codes)
     bvector_type universe_;
     size_type size_ = 0;
     unsigned n_planes_ = 0;

@@ -17,13 +17,17 @@ Signed vectors (``sparse_vector<int32_t / int64_t>`` and their RSC forms; ``from
 element as ``s2u(x)`` (src/bmbmatrix.h:2536-2569: ``x >= 0 -> x << 1``, ``x < 0 -> (-(x+1)) << 1 | 1``), so plane 0 is the
 sign plane.  Their searches take int64 values and run with ``F_SIGNED``; ``find_zero / find_nonzero`` stay unsigned searches
 for 0 over the same planes, which is what the reference computes for them (an OR of all planes).
+
+String vectors (``bm::str_sparse_vector<char, ...>``, ``StrSparseVector``) keep bit b of byte k of every element in plane 8k+b;
+``find_eq_str`` / ``find_eq_str_prefix`` / ``count_eq_str`` run as ``bmb200_scan_str`` (csrc/str_scan_kernel.cuh).  The numeric
+searches raise on a string vector.
 """
 from __future__ import annotations
 
 import numpy as np
 
 from . import capi
-from .capi import F_COUNT_ONLY, F_OPT_COMPRESS, F_SIGNED, SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT, SCAN_RANGE
+from .capi import F_COUNT_ONLY, F_OPT_COMPRESS, F_SIGNED, F_STR_PREFIX, SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT, SCAN_RANGE
 from .hostfmt import BLOCK_BITS, BVector, PackedSet, bits_to_words, result_to_bvector
 
 
@@ -120,6 +124,53 @@ class RscSparseVector:
         return BVector.from_words(bits_to_words(bits)).optimize()
 
 
+class StrSparseVector:
+    """``bm::str_sparse_vector<char, bvector<>, N>`` as the scanner sees it (not remapped): plane 8k+b holds bit b of byte k
+    of every element (``basic_bmatrix::set_octet``), ``rows_not_null()`` planes with the trailing empty ones trimmed, NULL
+    elements and positions >= size() all zero, and for a nullable vector the NOT-NULL plane."""
+
+    def __init__(self, planes: list[BVector], size: int, not_null: BVector | None = None):
+        self.planes = planes
+        self.size = int(size)
+        self.not_null = not_null
+        self.signed = False
+
+    @classmethod
+    def from_strings(cls, strs, null_mask=None, optimize: bool = True) -> "StrSparseVector":
+        """push_back(s) for every byte string [+ NULL where null_mask] + optimize()"""
+        bs = [bytes(x) for x in strs]
+        if any(b"\0" in b for b in bs):
+            raise ValueError("a string sparse vector holds C strings: no NUL inside a string")
+        n = len(bs)
+        nl = np.zeros(n, bool) if null_mask is None else np.asarray(null_mask, bool)
+        nb = max(1, (n + BLOCK_BITS - 1) // BLOCK_BITS)
+        width = max([len(b) for b, z in zip(bs, nl) if not z], default=0)
+        mat = np.zeros((nb * BLOCK_BITS, max(width, 1)), np.uint8)
+        for i, b in enumerate(bs):
+            if b and not nl[i]:
+                mat[i, :len(b)] = np.frombuffer(b, np.uint8)
+        used = np.bitwise_or.reduce(mat, axis=0)                       # which planes hold any bit
+        top = max([j + 1 for j in range(8 * width) if (used[j >> 3] >> (j & 7)) & 1], default=1)
+        planes = []
+        for j in range(top):
+            bits = (mat[:, j >> 3] >> np.uint8(j & 7)) & np.uint8(1)
+            bv = BVector.from_words(bits_to_words(bits))
+            planes.append(bv.optimize() if optimize else bv)
+        nn = None
+        if null_mask is not None:
+            bits = np.zeros(nb * BLOCK_BITS, np.uint8)
+            bits[:n] = ~nl
+            nn = BVector.from_words(bits_to_words(bits))
+            if optimize:
+                nn.optimize()
+        return cls(planes, n, nn)
+
+    def effective_slices(self) -> int:
+        return len(self.planes)
+
+    universe = SparseVector.universe
+
+
 class SparseVectorScanner:
     """``bm::sparse_vector_scanner<SV>`` bound to one vector (``bind``): the planes are packed and uploaded once, every
     search is one ``bmb200_scan`` launch.  Searches take one value or a list (a list = one batched launch, the
@@ -129,6 +180,7 @@ class SparseVectorScanner:
         self.ctx = ctx or capi.default_context()
         self.sv = sv
         self._rsc = isinstance(sv, RscSparseVector)
+        self._str = isinstance(sv, StrSparseVector)
         vecs = list(sv.planes) + [sv.universe()]
         if self._rsc:
             # one set as wide as the logical space: compressed planes (NULL past their columns), [0, effective_size), NN
@@ -151,14 +203,32 @@ class SparseVectorScanner:
 
     def _run(self, pred, values, count_only=False, signed=None):
         """signed: compare as signed values (default: the vector's signedness); find_zero / find_nonzero pass False"""
+        if self._str:
+            raise TypeError("numeric searches do not apply to a string vector: use find_eq_str / find_eq_str_prefix")
         signed = self.sv.signed if signed is None else signed
         single = np.ndim(values) == (1 if pred == SCAN_RANGE else 0)
         dt = np.int64 if signed else np.uint64
         vals = np.atleast_2d(np.asarray(values, dt)) if pred == SCAN_RANGE else np.atleast_1d(np.asarray(values, dt))
         flags = (F_COUNT_ONLY if count_only else F_OPT_COMPRESS) | (F_SIGNED if signed else 0)
         res = capi.scan(self.ctx, self._dset, pred, vals, 0, self.sv.effective_slices(), self._universe, flags, 0, self._scan_to)
+        return self._results(res, vals.shape[0], count_only, single)
+
+    def _run_str(self, strs, prefix, count_only=False):
+        if not self._str:
+            raise TypeError("string searches need a StrSparseVector")
+        single = isinstance(strs, (bytes, bytearray, str))
+        qs = [q.encode() if isinstance(q, str) else bytes(q) for q in ([strs] if single else strs)]
+        if any(b"\0" in q for q in qs):
+            raise ValueError("a query is a C string: no NUL inside it")
+        if not qs:
+            return []
+        flags = (F_COUNT_ONLY if count_only else F_OPT_COMPRESS) | (F_STR_PREFIX if prefix else 0)
+        res = capi.scan_str(self.ctx, self._dset, qs, 0, self.sv.effective_slices(), self._universe, flags)
+        return self._results(res, len(qs), count_only, single)
+
+    def _results(self, res, nv, count_only, single):
+        """a scan's result -> BVector per search (or its count); frees res"""
         try:
-            nv = vals.shape[0]
             if count_only:                 # rank decompression keeps the count: the totals of the compressed scan are the answer
                 t = [int(x) for x in res.group_totals(nv)]
                 return t[0] if single else t
@@ -190,3 +260,7 @@ class SparseVectorScanner:
     def count_gt(self, value):   return self._run(SCAN_GT, value, True)
     def count_range(self, lo, hi=None):
         return self._run(SCAN_RANGE, [lo, hi] if hi is not None else lo, True)
+    # string vectors: one query (bytes / str) or a list of them (one launch)
+    def find_eq_str(self, s):         return self._run_str(s, False)
+    def find_eq_str_prefix(self, s):  return self._run_str(s, True)
+    def count_eq_str(self, s):        return self._run_str(s, False, True)

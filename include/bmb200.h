@@ -23,6 +23,8 @@
  *   bmb200_set_upload_blobs       <- bm::deserialize / deserializer<BV>::deserialize  src/bmserial.h:4152,5578-6090
  *   bmb200_scan                   <- sparse_vector_scanner::find_eq/find_gt/find_ge/find_lt/find_le/find_range
  *                                                                   src/bmsparsevec_algo.h:1083-1182,2593-2632,4360-4395
+ *   bmb200_scan_str               <- sparse_vector_scanner::find_eq_str / find_eq_str_prefix / find_eq_str(TPipe&) over
+ *                                    str_sparse_vector            src/bmsparsevec_algo.h:2546-2588,3263-3436,4579-4651
  *   bmb200_rs_build               <- bvector::build_rs_index       src/bm.h:2531-2660, rs_index src/bmrs.h:688-715
  *   bmb200_rank_batch             <- bvector::count_to             src/bm.h:3120-3167
  *   bmb200_select_batch           <- bvector::select               src/bm.h:5350-5385
@@ -359,6 +361,30 @@ typedef struct bmb200_scan_args {
     uint32_t        nb_to;      /* 0 == n_blocks */
 } bmb200_scan_args;
 int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* args, bmb200_result** inout);
+
+/* String searches over ONE string sparse vector (bm::str_sparse_vector<char, ...>, src/bmstrsparsevec.h): plane 8k+b (bit b of
+ * byte k of every element, basic_bmatrix::set_octet src/bmbmatrix.h:1571) is set vector plane0 + 8k + b, for the rows
+ * [0, rows_not_null()).  For a query s of length L (its slot holds a C string) and the universe U:
+ *   exact (find_eq_str, src/bmsparsevec_algo.h:3372-3419):  U & {i : every plane j matches bit j of s zero-padded}
+ *   BMB200_F_STR_PREFIX (find_eq_str_prefix, :3263):          the same over the planes j < 8L only
+ *   L == 0, either mode (find_zero, :3412-3416):              U & {i : every plane is 0}
+ * A query with a 1-bit at a plane >= n_planes matches nothing (the get_slice_mask pre-screen, :2569-2570).  One launch answers
+ * n_values queries; the result is value-major like bmb200_scan (per-query cardinalities through bmb200_result_group_totals).
+ * Remapped vectors (is_remap()) are searched with the remapped codes of the query (str_sparse_vector::remap_tosv); the
+ * remap tables stay with the caller. */
+#define BMB200_F_STR_PREFIX 16u   /* bmb200_scan_str only: compare the first strlen(s) bytes (find_eq_str_prefix) */
+typedef struct bmb200_scan_str_args {
+    uint32_t    plane0;      /* plane 8k+b (bit b of byte k) = set vector plane0 + 8k + b */
+    uint32_t    n_planes;    /* 1..2048 (str_sparse_vector rows_not_null())                 */
+    uint32_t    universe;    /* as bmb200_scan: NOT-NULL plane / [0,size) vector / 0xffffffff */
+    uint32_t    flags;       /* BMB200_F_COUNT_ONLY / BMB200_F_OPT_COMPRESS | BMB200_F_STR_PREFIX */
+    const char* strs;        /* HOST: n_values strings, stride bytes each, NUL-padded        */
+    uint32_t    stride;      /* bytes per string slot                                        */
+    uint32_t    n_values;
+    uint32_t    nb_from, nb_to;
+} bmb200_scan_str_args;
+/* BMB200_ERR_BADARG also for n_planes > 2048 and for a slot without a NUL */
+int bmb200_scan_str(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_str_args* args, bmb200_result** inout);
 
 /* end-to-end convenience: HOST packed set in, HOST metadata out, in one call: H2D of the whole set (every call), kernel,
  * D2H of the per-column metadata requested in meta_out (kind / popcnt / digest / nruns) and of the cardinality.  The result
