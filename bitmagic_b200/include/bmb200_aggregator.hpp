@@ -78,11 +78,29 @@ struct tree_view
     }
 };
 
-template<class BV>
-uint32_t blocks_of(const BV& bv)
+/// block columns of a `size`-bit range, as a 64-bit count: 2^32 for a default-constructed BM64ADDR vector (size 2^48 - 1)
+inline uint64_t size_blocks(uint64_t size) { return (size + 65535ull) >> 16; }
+
+/// a block-column count as the u32 the C ABI takes.  Only a BM64ADDR vector can need more (a bit in its last block, 65536 *
+/// (2^32 - 1) and up): refused, never truncated
+inline uint32_t column_count(uint64_t n_cols, const char* what)
 {
-    typename BV::size_type sz = bv.size();
-    return (uint32_t)((uint64_t(sz) + 65535ull) >> 16);
+    if (n_cols > 0xFFFFFFFFull)
+        throw std::length_error(std::string(what) + ": " + std::to_string(n_cols) + " block columns do not fit the 32-bit column count of libbmb200");
+    return (uint32_t)n_cols;
+}
+
+/// block columns [0, extent) that hold every set bit of bv: up to its last set bit (find_reverse), capped by size(); one column
+/// for an empty vector of non-zero size, none for size() == 0.  A default-constructed vector spans size() = 2^32 bits (32-bit
+/// build) or 2^48 - 1 bits (BM64ADDR): only its populated extent is uploaded.
+template<class BV>
+uint32_t extent_of(const BV& bv)
+{
+    const uint64_t cap = size_blocks(uint64_t(bv.size()));
+    uint64_t n = 1;
+    typename BV::size_type last = 0;
+    if (bv.get_blocks_manager().is_init() && bv.find_reverse(last)) n = (uint64_t(last) >> 16) + 1u;
+    return column_count(std::min(n, cap), "bm::b200: vector extent");
 }
 
 /// store a fetched result (per-column flat form) into the target through the public block manager.  The target is REPLACED
@@ -281,14 +299,15 @@ public:
     ~device_set() { release(); }
     device_set(const device_set&) = delete; device_set& operator=(const device_set&) = delete;
 
-    /// (re)build the device copy from n vectors; nb_to != 0 uploads only the block columns [nb_from, nb_to) (one rank's shard)
+    /// (re)build the device copy from n vectors; nb_to != 0 uploads only the block columns [nb_from, nb_to) (one rank's shard),
+    /// which may reach past the vectors' populated extent up to their size()
     void assign(const BV* const* vecs, size_t n, uint32_t nb_from = 0, uint32_t nb_to = 0)
     {
         release();
         if (!n) return;
-        uint32_t nblk = 0;
-        for (size_t k = 0; k < n; ++k) nblk = std::max(nblk, detail::blocks_of(*vecs[k]));
-        if (nb_to && nb_to < nblk) nblk = nb_to;
+        uint32_t nblk = 0; uint64_t cap = 0;
+        for (size_t k = 0; k < n; ++k) { nblk = std::max(nblk, detail::extent_of(*vecs[k])); cap = std::max(cap, detail::size_blocks(vecs[k]->size())); }
+        if (nb_to) nblk = (uint32_t)std::min<uint64_t>(nb_to, cap);
         if (nb_from >= nblk) throw std::range_error("device_set: empty block range");
         nb_from_ = nb_from; n_blocks_ = nblk - nb_from;
         std::vector<detail::tree_view<BV>> views; std::vector<bmb200_vec_blocks> vb;
@@ -589,10 +608,11 @@ private:
         for (size_t k = 0; k < n0 + n1; ++k)
         {
             all[k] = k < n0 ? s0[k] : s1[k - n0];
-            uint32_t nb = detail::blocks_of(*all[k]);
+            uint32_t nb = detail::extent_of(*all[k]);
             if (nb > n_blocks_) n_blocks_ = nb;
         }
-        if (spare_blocks_ && n_blocks_ < 65536u) n_blocks_ += spare_blocks_;
+        if (spare_blocks_ && n_blocks_ < detail::size_blocks(max_size_))
+            n_blocks_ = detail::column_count(uint64_t(n_blocks_) + spare_blocks_, "bm::b200::aggregator");
         detail::set_uploader<BV> up;
         up.begin(ctx_.get(), n0 + n1);
         detail::build_views(all.data(), all.size(), 0u, n_blocks_, views_, vb_);
@@ -672,7 +692,7 @@ public:
     void assign(const BV* const* vecs, size_t n)
     {
         uint32_t nblk = 0;
-        for (size_t k = 0; k < n; ++k) nblk = std::max(nblk, detail::blocks_of(*vecs[k]));
+        for (size_t k = 0; k < n; ++k) nblk = std::max(nblk, detail::extent_of(*vecs[k]));
         n_blocks_ = nblk; widest_ = 0;
         for (int r = 0; r < nranks_; ++r) { uint32_t a, b; check(bmb200_shard_range(nblk, nranks_, r, &a, &b), "bmb200_shard_range"); widest_ = std::max(widest_, b - a); }
         check(bmb200_shard_range(nblk, nranks_, rank_, &from_, &to_), "bmb200_shard_range");
@@ -764,7 +784,7 @@ public:
         }
         if (!ng || uniq.empty()) return;
         uint32_t n_blocks = 0; size_type max_size = 0;
-        for (const BV* bv : uniq) { n_blocks = std::max(n_blocks, detail::blocks_of(*bv)); if (bv->size() > max_size) max_size = bv->size(); }
+        for (const BV* bv : uniq) { n_blocks = std::max(n_blocks, detail::extent_of(*bv)); if (bv->size() > max_size) max_size = bv->size(); }
         std::vector<detail::tree_view<BV>> views(uniq.size()); std::vector<bmb200_vec_blocks> vb(uniq.size());
         for (size_t k = 0; k < uniq.size(); ++k) {
             views[k].build(*uniq[k], n_blocks);
@@ -829,7 +849,7 @@ void binop(context& c, int op, BV& t, const BV& a, const BV& b, typename BV::opt
     { set = ds->handle(); ia = (uint32_t)ds->index_of(&a); ib = (uint32_t)ds->index_of(&b); n_blocks = ds->n_blocks(); nb_off = ds->nb_from(); own = false; }
     else
     {
-        n_blocks = std::max(detail::blocks_of(a), detail::blocks_of(b));
+        n_blocks = std::max(detail::extent_of(a), detail::extent_of(b));
         if (!n_blocks) { t.clear(true); return; }
         std::vector<detail::tree_view<BV>> views; std::vector<bmb200_vec_blocks> vb;
         detail::build_views(both, 2, 0u, n_blocks, views, vb);
@@ -857,12 +877,19 @@ template<class BV> void bit_xor(context& c, BV& t, const BV& a, const BV& b, typ
 /// aggregator::combine_or / combine_and_sub (src/bmaggregator.h:1101,1162); bm::operation_deserializer<BV> (src/bmserial.h:1070)
 /// is the reference's own one-BLOB-at-a-time form of "operate on a BLOB without keeping the vector".
 /// `size` = size() of the serialized vectors (the result is resized to it, like resize_target does with max(source sizes)).
+/// `extent` (0 = `size`): a bound the caller knows for the BLOBs' set bits -- every set bit lies below it; the BLOBs are decoded
+/// into block columns [0, ceil(min(extent, size) / 65536)), and blocks past them are not read.  The BLOBs are never decoded on
+/// the host, so this binding cannot find their populated extent itself.  A default-constructed BM64ADDR vector has size()
+/// 2^48 - 1, which would need 2^32 columns, one more than the C ABI's u32 column count: its BLOBs need an `extent`, and without
+/// one the constructor throws std::length_error.
 template<class BV>
 class blob_aggregator
 {
 public:
     typedef typename BV::size_type size_type;
-    blob_aggregator(context& c, size_type size) : ctx_(c), size_(size), n_blocks_((uint32_t)((uint64_t(size) + 65535ull) >> 16)) {}
+    blob_aggregator(context& c, size_type size, size_type extent = 0)
+        : ctx_(c), size_(size),
+          n_blocks_(detail::column_count(detail::size_blocks(extent && extent < size ? extent : size), "bm::b200::blob_aggregator (pass the BLOBs' extent)")) {}
     void set_optimization(typename BV::optmode opt = BV::opt_compress) { opt_mode_ = opt; }
     /// attach a BLOB (not owned) to group 0 (OR / AND sources) or group 1 (SUB sources), like aggregator::add(bv, group)
     size_t add(const unsigned char* buf, size_t buf_size, unsigned group = 0) { bmb200_blob b{buf, (uint64_t)buf_size}; grp_[group ? 1 : 0].push_back(b); return grp_[group ? 1 : 0].size(); }
@@ -936,7 +963,7 @@ void build_rs_index(context& c, const BV& bv, typename BV::rs_index_type* rs)
     rs->set_total((typename BV::block_idx_type)(nb + 1));
     rs->resize((typename BV::block_idx_type)(nb + 1));
     rs->resize_effective_super_blocks(real_top);
-    uint32_t n_blocks = max_top * 256u;
+    uint32_t n_blocks = detail::column_count(uint64_t(max_top) * 256u, "bm::b200::build_rs_index");
     detail::tree_view<BV> view; view.build(bv, n_blocks);
     bmb200_vec_blocks vb{n_blocks, view.kind.data(), view.ptr.data()};
     bmb200_set* set = nullptr; bmb200_rs* drs = nullptr;

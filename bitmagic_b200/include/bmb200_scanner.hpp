@@ -63,13 +63,13 @@ public:
             n_planes_ = sv.effective_slices();
             while (n_planes_ > 1 && !sv.get_slice(n_planes_ - 1)) --n_planes_;
         }
-        n_blocks_ = (uint32_t)((uint64_t(size_) + 65535ull) >> 16); if (!n_blocks_) n_blocks_ = 1;
+        n_blocks_ = detail::column_count(std::max<uint64_t>(detail::size_blocks(size_), 1u), "bm::b200::scanner");
         const bvector_type* nn = sv.get_null_bvector();
         uint32_t n_vec = n_planes_ + 1;
         if constexpr (SV::is_compressed()) {
             // compressed planes: positions [0, effective_size()); the universe is that range, NN maps it to the logical space
             const size_type eff = sv.effective_size();
-            scan_to_ = (uint32_t)((uint64_t(eff) + 65535ull) >> 16); if (!scan_to_) scan_to_ = 1;
+            scan_to_ = detail::column_count(std::max<uint64_t>(detail::size_blocks(eff), 1u), "bm::b200::scanner");
             universe_.clear(true); if (eff) universe_.set_range(0, eff - 1); universe_.optimize();
             n_vec = n_planes_ + 2;
         } else {
@@ -298,14 +298,9 @@ public:
     }
 
 private:
-    static uint32_t extent(const BV& bv)                              // block columns up to the last set bit
-    {
-        typename BV::size_type last = 0;
-        return bv.find_reverse(last) ? (uint32_t)(uint64_t(last) >> 16) + 1u : 0u;
-    }
     void call(BV& bv_target, const BV& bv_idx, const BV& bv_src, bool comp)
     {
-        uint32_t n_blocks = std::max(extent(bv_idx), extent(bv_src)); if (!n_blocks) n_blocks = 1;
+        uint32_t n_blocks = std::max(detail::extent_of(bv_idx), detail::extent_of(bv_src)); if (!n_blocks) n_blocks = 1;
         const BV* both[2] = {&bv_idx, &bv_src};
         std::vector<detail::tree_view<BV>> views(2); std::vector<bmb200_vec_blocks> vb(2);
         for (int k = 0; k < 2; ++k) {

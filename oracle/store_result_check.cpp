@@ -15,9 +15,37 @@ int main()
 {
     std::mt19937 rng(7);
     bvect target; int fails = 0;
+#ifdef BM64ADDR
+    // the binding's upload extent (bm::b200::detail::extent_of): populated blocks up to the last set bit, capped by size(), never
+    // truncated to 32 bits; a vector whose last block is column 2^32 - 1 needs 2^32 columns and is refused
+    {
+        const uint64_t G = uint64_t(1) << 32;
+        auto extent_with = [](uint64_t bit) { bvect bv; bv.set((bvect::size_type)bit); return (uint64_t)bm::b200::detail::extent_of(bv); };
+        bvect empty, sized(1000), none(0);
+        struct { const char* what; uint64_t got, want; } cases[] = {
+            {"default vector", bm::b200::detail::extent_of(empty), 1}, {"size 1000", bm::b200::detail::extent_of(sized), 1},
+            {"size 0", bm::b200::detail::extent_of(none), 0}, {"bit 2^32 - 1", extent_with(G - 1), 65536},
+            {"bit 2^32", extent_with(G), 65537}, {"bit 2^33", extent_with(2 * G), 131073},
+            {"bit 2^32 + 65535", extent_with(G + 65535), 65537}, {"bit 2^32 + 65536", extent_with(G + 65536), 65538},
+            {"default size in blocks", bm::b200::detail::size_blocks(empty.size()), G}};
+        for (const auto& c : cases)
+            if (c.got != c.want) { ++fails; std::printf("extent %s: %llu, want %llu\n", c.what, (unsigned long long)c.got, (unsigned long long)c.want); }
+        bool refused = false;
+        try { extent_with(empty.size() - 1); } catch (const std::length_error&) { refused = true; }
+        if (!refused) { ++fails; std::printf("extent of a bit in block 2^32 - 1 was not refused\n"); }
+        refused = false;
+        try { bm::b200::detail::column_count(G, "column_count"); } catch (const std::length_error&) { refused = true; }
+        if (!refused || bm::b200::detail::column_count(G - 1, "column_count") != G - 1) { ++fails; std::printf("column_count(2^32) not refused\n"); }
+    }
+#endif
     for (int it = 0; it < 60; ++it) {
         const uint32_t n_cols = (it % 3 == 0) ? 2400 : (it % 3 == 1 ? 700 : 2048 + 256 * (it % 5));
+#ifdef BM64ADDR
+        // shard offsets past 2^32 bits: top-level index >= 256, one of them straddling top-level entries 255 / 256
+        const uint32_t nb_off = (it % 4 == 3) ? 100 : (it % 4 == 2 ? 65536u + 300u : (it % 4 == 1 ? 65536u - 600u : 0));
+#else
         const uint32_t nb_off = (it % 4 == 3) ? 100 : 0;
+#endif
         std::vector<uint8_t> kind(n_cols); std::vector<uint64_t> off(n_cols);
         std::vector<uint16_t> gaps; std::vector<uint32_t> bits;
         const int mode = it % 6;
@@ -36,7 +64,8 @@ int main()
                 gaps.insert(gaps.end(), g.begin(), g.end()); while (gaps.size() % 8) gaps.push_back(0);
             }
         }
-        const bvect::size_type sz = (bvect::size_type)((it % 7 == 6 ? 3000u : 2700u) * 65536u - 1);
+        bvect::size_type sz = (bvect::size_type)((it % 7 == 6 ? 3000u : 2700u) * 65536u - 1);
+        if (nb_off >= 65536u - 600u) sz = (bvect::size_type)((uint64_t(nb_off) + n_cols + (it % 7 == 6 ? 5u : 0u)) * 65536u - 1u);
         bvect fresh;
         bm::b200::detail::store_result(fresh, sz, n_cols, kind.data(), off.data(), bits.data(), gaps.data(), nb_off);
         bm::b200::detail::store_result(target, sz, n_cols, kind.data(), off.data(), bits.data(), gaps.data(), nb_off);

@@ -32,6 +32,234 @@ static void fill(bvect& bv, std::mt19937_64& rng, unsigned n_bits, double densit
     }
 }
 
+#ifdef BM64ADDR
+// ---- BM64ADDR: vectors past 2^32 bits.  Their blocks straddle columns 65535 / 65536 (bit 2^32) and reach block 69999, so every
+// upload holds ~70 000 columns; a default-constructed vector is 2^48 - 1 bits long, which the binding must not upload whole ----
+static const uint64_t B = 65536u, G = uint64_t(1) << 32;
+
+// shape 0: random bits in a few block spans; 1: plus a run of FULL blocks across 2^32; 2: plus the two bits around 2^32;
+// 3: GAP-friendly runs only
+static void fill64(bvect& bv, std::mt19937_64& rng, double density, int shape)
+{
+    const uint64_t spans[][2] = {{0, 2}, {65531, 65541}, {66600, 66601}, {69996, 70000}};
+    std::geometric_distribution<unsigned> skip(density);
+    if (shape != 3)
+        for (const auto& s : spans)
+            for (uint64_t p = s[0] * B + skip(rng); p < s[1] * B; p += 1 + skip(rng)) bv.set_bit_no_check((bvect::size_type)p);
+    if (shape == 1) bv.set_range(G - 3 * B - 77, G + 2 * B + 500);
+    if (shape == 2) { bv.set_bit(G - 1); bv.set_bit(G); bv.set_bit(70000 * B - 1); }
+    if (shape == 3)
+        for (uint64_t p = 65533 * B + 11; p < 65540 * B; p += 4099 + (rng() % 2000)) bv.set_range(p, p + (rng() % 300));
+}
+
+static bool same_kinds(const bvect& a, const bvect& b)
+{
+    bvect::statistics s1, s2; a.calc_stat(&s1); b.calc_stat(&s2);
+    return s1.bit_blocks == s2.bit_blocks && s1.gap_blocks == s2.gap_blocks;
+}
+
+static void check_past_2_32(bm::b200::context& ctx, std::mt19937_64& rng)
+{
+    std::vector<std::unique_ptr<bvect>> vs;
+    for (int k = 0; k < 10; ++k) {
+        vs.emplace_back(new bvect());
+        fill64(*vs.back(), rng, k < 6 ? 0.6 / (k + 1) : 0.02, k % 4);
+        if (k >= 4) { BM_DECLARE_TEMP_BLOCK(tb) vs.back()->optimize(tb, bvect::opt_compress); }
+    }
+    std::vector<const bvect*> all; for (auto& v : vs) all.push_back(v.get());
+    for (int opt = 0; opt < 2; ++opt) {
+        const bvect::optmode om = opt ? bvect::opt_compress : bvect::opt_none;
+        bm::aggregator<bvect> ref; ref.set_optimization(om);
+        bm::b200::aggregator<bvect> gpu(ctx); gpu.set_optimization(om);
+        for (size_t n : {size_t(2), size_t(5), all.size()}) {
+            bvect r, g;
+            ref.combine_or(r, all.data(), n); gpu.combine_or(g, all.data(), n);
+            CHECK(r.compare(g) == 0 && r.count() == g.count() && (!opt || same_kinds(r, g)), "64: combine_or n=%zu opt=%d (%llu vs %llu bits)",
+                  n, opt, (unsigned long long)r.count(), (unsigned long long)g.count());
+            ref.combine_and(r, all.data(), n); gpu.combine_and(g, all.data(), n);
+            CHECK(r.compare(g) == 0 && r.count() == g.count(), "64: combine_and n=%zu opt=%d", n, opt);
+        }
+        for (size_t na : {size_t(1), size_t(2)}) {
+            bvect r, g;
+            bool f1 = ref.combine_and_sub(r, all.data(), na, all.data() + na, all.size() - na, false);
+            bool f2 = gpu.combine_and_sub(g, all.data(), na, all.data() + na, all.size() - na, false);
+            CHECK(f1 == f2 && r.compare(g) == 0 && r.count() == g.count() && same_kinds(r, g), "64: combine_and_sub na=%zu opt=%d", na, opt);
+            CHECK(gpu.count_and_sub(all.data(), na, all.data() + na, all.size() - na) == r.count(), "64: count_and_sub na=%zu", na);
+        }
+        for (size_t n : {size_t(1), size_t(2), size_t(3)}) {     // dense sources: the carry crosses column 65535 -> 65536
+            const bvect* sh[3] = {all[1], all[0], all[2]};
+            bvect r, g;
+            bool f1 = ref.combine_shift_right_and(r, sh, n, false), f2 = gpu.combine_shift_right_and(g, sh, n, false);
+            CHECK(f1 == f2 && r.compare(g) == 0 && r.count() == g.count(), "64: combine_shift_right_and n=%zu opt=%d (%llu vs %llu bits)",
+                  n, opt, (unsigned long long)r.count(), (unsigned long long)g.count());
+        }
+    }
+    {   // find_first_and_sub: answers past 2^32, with and without range hints above 2^32, uploaded and resident
+        bvect a1, a2, s1;
+        a1.set_range(G + 5 * B + 100, G + 5 * B + 4000); a1.set_range(G - 20, G + 10); a1.set_bit(3 * B);
+        a2.set_range(G + 5 * B + 300, G + 6 * B); a2.set_range(G - 5, G + 3);
+        s1.set_range(G - 30, G - 1); s1.set_bit(3 * B);
+        bm::b200::device_set<bvect> ds(ctx);
+        std::vector<const bvect*> mem = {&a1, &a2, &s1, all[0], all[1], all[2]};
+        ds.assign(mem.data(), mem.size());
+        std::vector<std::vector<const bvect*>> ands = {{&a1, &a2}, {all[0], all[1]}, {all[2]}};
+        std::vector<std::vector<const bvect*>> subs = {{}, {&s1}, {all[2]}};
+        struct Hint { bool on; uint64_t from, to; };
+        const Hint hints[] = {{false, 0, 0}, {true, G - 3 * B, G + 9 * B}, {true, G + 1, G + 2 * B + 17}, {true, G + 5 * B + 250, G + 5 * B + 3999},
+                              {true, G + 5 * B + 4001, G + 5 * B + 9000}, {true, 65535 * B + 5, 65535 * B + 65535}, {true, 69990 * B, 70000 * B - 1}};
+        bm::aggregator<bvect> ref; bm::b200::aggregator<bvect> gpu(ctx);
+        for (int resident = 0; resident < 2; ++resident) {
+            gpu.set_device_set(resident ? &ds : nullptr);
+            for (const Hint& h : hints)
+                for (size_t x = 0; x < ands.size(); ++x) for (size_t y = 0; y < subs.size(); ++y) {
+                    ref.reset_range_hint(); gpu.reset_range_hint();
+                    if (h.on) { bool r1 = ref.set_range_hint(h.from, h.to), r2 = gpu.set_range_hint(h.from, h.to); CHECK(r1 == r2, "64: set_range_hint return"); }
+                    bvect::size_type i1 = 0, i2 = 0;
+                    bool f1 = ref.find_first_and_sub(i1, ands[x].data(), ands[x].size(), subs[y].empty() ? 0 : subs[y].data(), subs[y].size());
+                    bool f2 = gpu.find_first_and_sub(i2, ands[x].data(), ands[x].size(), subs[y].empty() ? 0 : subs[y].data(), subs[y].size());
+                    CHECK(f1 == f2 && (!f1 || i1 == i2), "64: find_first_and_sub and=%zu sub=%zu hint=[%llu,%llu] resident=%d: ref %d@%llu vs %d@%llu",
+                          x, y, (unsigned long long)h.from, (unsigned long long)h.to, resident, (int)f1, (unsigned long long)i1, (int)f2, (unsigned long long)i2);
+                }
+        }
+        bvect::size_type i1 = 0, i2 = 0;
+        ref.reset_range_hint(); gpu.reset_range_hint(); gpu.set_device_set(nullptr);
+        const bvect* aa[2] = {&a1, &a2};
+        bool f1 = ref.find_first_and_sub(i1, aa, 2, 0, 0), f2 = gpu.find_first_and_sub(i2, aa, 2, 0, 0);
+        CHECK(f1 && f2 && i1 == i2 && i2 == G - 5, "64: find_first_and_sub straddling 2^32: %llu", (unsigned long long)i2);
+    }
+    {   // 3-operand ops, bits and block kinds
+        std::vector<const bvect*> ops = {all[0], all[1], all[3], all[5], all[6], all[7]};
+        for (int opt = 0; opt < 2; ++opt) {
+            const bvect::optmode om = opt ? bvect::opt_compress : bvect::opt_none;
+            for (size_t x = 0; x < ops.size(); ++x) for (size_t y = 0; y < ops.size(); ++y) {
+                if (x == y) continue;
+                for (int op = 0; op < 4; ++op) {
+                    bvect t1, t2;
+                    switch (op) {
+                    case 0: t1.bit_and(*ops[x], *ops[y], om); bm::b200::bit_and(ctx, t2, *ops[x], *ops[y], om); break;
+                    case 1: t1.bit_or (*ops[x], *ops[y], om); bm::b200::bit_or (ctx, t2, *ops[x], *ops[y], om); break;
+                    case 2: t1.bit_sub(*ops[x], *ops[y], om); bm::b200::bit_sub(ctx, t2, *ops[x], *ops[y], om); break;
+                    default: t1.bit_xor(*ops[x], *ops[y], om); bm::b200::bit_xor(ctx, t2, *ops[x], *ops[y], om); break;
+                    }
+                    CHECK(t1.compare(t2) == 0 && t1.count() == t2.count() && same_kinds(t1, t2), "64: binop %d (%zu,%zu) opt=%d", op, x, y, opt);
+                }
+            }
+        }
+    }
+    {   // pipeline with an OR target
+        bm::aggregator<bvect> ref; bm::b200::aggregator<bvect> gpu(ctx);
+        bm::aggregator<bvect>::pipeline<bm::agg_opt_bvect_and_counts> rp;
+        bm::b200::pipeline<bvect> gp(ctx);
+        bvect or_ref, or_gpu; or_ref.init(); or_gpu.init();
+        rp.set_or_target(&or_ref); gp.set_or_target(&or_gpu);
+        for (int g = 0; g < 6; ++g) {
+            auto* a1 = rp.add(); auto* a2 = gp.add();
+            for (int k = 0; k < 1 + g % 2; ++k) { a1->add(all[(g + k) % 10], 0); a2->add(all[(g + k) % 10], 0); }
+            for (int k = 0; k < g % 3; ++k) { a1->add(all[(g * 3 + k + 4) % 10], 1); a2->add(all[(g * 3 + k + 4) % 10], 1); }
+        }
+        rp.complete(); gp.complete();
+        ref.combine_and_sub(rp); gpu.combine_and_sub(gp);
+        auto& r1 = rp.get_bv_res_vector(); auto& c1 = rp.get_bv_count_vector();
+        auto& r2 = gp.get_bv_res_vector(); auto& c2 = gp.get_bv_count_vector();
+        CHECK(r1.size() == r2.size() && c1.size() == c2.size(), "64: pipeline sizes");
+        for (size_t g = 0; g < r2.size() && g < r1.size(); ++g) {
+            CHECK((uint64_t)c1[g] == (uint64_t)c2[g] && (r1[g] == 0) == (r2[g] == 0) && (!r1[g] || !r2[g] || r1[g]->compare(*r2[g]) == 0), "64: pipeline g=%zu", g);
+        }
+        CHECK(or_ref.compare(or_gpu) == 0, "64: pipeline OR target");
+    }
+    {   // resident device_set, and a shard of columns [65530, 65540) around 2^32
+        bm::b200::device_set<bvect> ds(ctx);
+        ds.assign(all.data(), all.size());
+        CHECK(ds.n_blocks() == 70000u, "64: device_set columns %u (want 70000)", ds.n_blocks());
+        bm::aggregator<bvect> ref; ref.set_optimization(bvect::opt_compress);
+        bm::b200::aggregator<bvect> gpu(ctx); gpu.set_optimization(bvect::opt_compress); gpu.set_device_set(&ds);
+        bvect r, g;
+        ref.combine_or(r, all.data(), all.size()); gpu.combine_or(g, all.data(), all.size());
+        CHECK(r.compare(g) == 0 && same_kinds(r, g), "64: resident combine_or");
+        bool f1 = ref.combine_and_sub(r, all.data(), 2, all.data() + 2, all.size() - 2, false);
+        bool f2 = gpu.combine_and_sub(g, all.data(), 2, all.data() + 2, all.size() - 2, false);
+        CHECK(f1 == f2 && r.compare(g) == 0, "64: resident combine_and_sub");
+        bm::b200::device_set<bvect> sh(ctx);
+        sh.assign(all.data(), all.size(), 65530, 65540);
+        bm::b200::aggregator<bvect> g2(ctx); g2.set_optimization(bvect::opt_compress); g2.set_device_set(&sh);
+        ref.combine_or(r, all.data(), all.size()); g2.combine_or(g, all.data(), all.size());
+        bvect mask; mask.set_range(65530 * B, 65540 * B - 1);
+        r &= mask;
+        CHECK(r.compare(g) == 0 && r.count() == g.count(), "64: shard [65530,65540)");
+    }
+    // rs_index built on the GPU, queried by the reference's count_to / select past 2^32
+    for (int k : {0, 1, 2, 7}) {
+        const bvect& bv = *all[k];
+        bvect::rs_index_type rs_ref, rs_gpu;
+        bv.build_rs_index(&rs_ref);
+        bm::b200::build_rs_index(ctx, bv, &rs_gpu);
+        CHECK(rs_ref.count() == rs_gpu.count(), "64: rs count k=%d", k);
+        bool q = true;
+        const uint64_t fixed[] = {0, G - 1, G, G + 1, 65536 * B + 65535, 66600 * B + 3, 70000 * B - 1, 70000 * B, 80000 * B};
+        for (int i = 0; i < 20000; ++i) {
+            bvect::size_type p = i < 9 ? (bvect::size_type)fixed[i] : (bvect::size_type)(i % 2 ? G - 6 * B + rng() % (12 * B) : rng() % (70000 * B));
+            q &= bv.count_to(p, rs_gpu) == bv.count_to(p, rs_ref);
+            bvect::size_type r = (bvect::size_type)(rng() % (rs_ref.count() + 2)), p1 = 0, p2 = 0;
+            bool f1 = bv.select(r, p1, rs_ref), f2 = bv.select(r, p2, rs_gpu);
+            q &= (f1 == f2) && (!f1 || p1 == p2);
+        }
+        CHECK(q, "64: rank/select with the GPU-built index k=%d", k);
+    }
+    // sparse_vector<unsigned> of more than 2^32 elements: values around 2^32, plain (universe [0, size)) and nullable
+    for (int nullable = 0; nullable < 2; ++nullable) {
+        typedef bm::sparse_vector<unsigned, bvect> svect;
+        svect sv(nullable ? bm::use_null : bm::no_null);
+        sv.resize((svect::size_type)(G + 2 * B + 99));
+        for (uint64_t i = G - 2 * B + 5; i < G + 2 * B + 99; ++i) {
+            if (nullable && rng() % 7 == 0) continue;
+            unsigned v = rng() % 3 == 0 ? 0u : unsigned(rng() % 900);
+            if (i >= G - 300 && i < G + 700) v = 55;
+            sv.set((svect::size_type)i, v);
+        }
+        for (uint64_t i = 0; i < 3000; ++i) sv.set((svect::size_type)(i * 7), unsigned(i % 60));
+        { BM_DECLARE_TEMP_BLOCK(tb) sv.optimize(tb); }
+        bm::sparse_vector_scanner<svect> ref_sc;
+        bm::b200::scanner<svect> gpu_sc(ctx, sv);
+        for (unsigned v : {0u, 55u, 899u, 1000u}) {
+            bvect a, b;
+            ref_sc.find_eq(sv, v, a); gpu_sc.find_eq(v, b); CHECK(a.compare(b) == 0 && a.count() == b.count(), "64: scanner find_eq(%u) nullable=%d", v, nullable);
+            ref_sc.find_gt(sv, v, a); gpu_sc.find_gt(v, b); CHECK(a.compare(b) == 0, "64: scanner find_gt(%u) nullable=%d", v, nullable);
+            ref_sc.find_le(sv, v, a); gpu_sc.find_le(v, b); CHECK(a.compare(b) == 0 && a.count() == b.count(), "64: scanner find_le(%u) nullable=%d", v, nullable);
+            ref_sc.find_range(sv, v / 2, v, a); gpu_sc.find_range(v / 2, v, b); CHECK(a.compare(b) == 0, "64: scanner find_range(%u) nullable=%d", v, nullable);
+        }
+        std::vector<uint64_t> vals = {7, 55, 0};
+        std::vector<bvect> outs; std::vector<bvect::size_type> cnts;
+        gpu_sc.find_batch(BMB200_SCAN_EQ, vals, outs); gpu_sc.count_batch(BMB200_SCAN_EQ, vals, cnts);
+        for (size_t k = 0; k < vals.size(); ++k) {
+            bvect a; ref_sc.find_eq(sv, (unsigned)vals[k], a);
+            CHECK(a.compare(outs[k]) == 0 && a.count() == cnts[k], "64: scanner batch eq k=%zu nullable=%d", k, nullable);
+        }
+    }
+    // serialization BLOBs of these vectors (64-bit stream headers, blocks past 65535), decoded and aggregated on the GPU
+    for (unsigned level : {2u, 6u}) {
+        std::vector<bm::serializer<bvect>::buffer> bufs(all.size());
+        for (size_t k = 0; k < all.size(); ++k) { bm::serializer<bvect> ser; ser.set_compression_level(level); ser.serialize(*all[k], bufs[k]); }
+        bm::aggregator<bvect> ref; ref.set_optimization(bvect::opt_compress);
+        // the sources' own size (2^48 - 1: default vectors) and the bound of their bits, which a BLOB reader has to be told
+        bm::b200::blob_aggregator<bvect> gpu(ctx, all[0]->size(), (bvect::size_type)(70000 * B)); gpu.set_optimization(bvect::opt_compress);
+        for (size_t k = 0; k < all.size(); ++k) gpu.add(bufs[k].data(), bufs[k].size(), k < 2 ? 0 : 1);
+        bvect r, g;
+        bool f1 = ref.combine_and_sub(r, all.data(), 2, all.data() + 2, all.size() - 2, false), f2 = gpu.combine_and_sub(g);
+        CHECK(f1 == f2 && r.compare(g) == 0 && r.count() == g.count(), "64: blob combine_and_sub level=%u", level);
+        gpu.reset();
+        for (size_t k = 0; k < all.size(); ++k) gpu.add(bufs[k].data(), bufs[k].size());
+        ref.combine_or(r, all.data(), all.size()); gpu.combine_or(g);
+        CHECK(r.compare(g) == 0 && r.count() == g.count() && r.size() == g.size(), "64: blob combine_or level=%u", level);
+    }
+    {   // without an extent, a default vector's size needs 2^32 columns: refused, not truncated to 0
+        bool refused = false;
+        try { bm::b200::blob_aggregator<bvect> gpu(ctx, bvect().size()); } catch (const std::length_error&) { refused = true; }
+        CHECK(refused, "64: blob_aggregator of size 2^48 - 1 without an extent");
+    }
+    bmb200_ctx_trim(ctx.get());
+}
+#endif
+
 int main()
 {
     std::mt19937_64 rng(20260923);
@@ -361,6 +589,9 @@ int main()
             CHECK(t_ref.compare(t_gpu) == 0 && t_ref.count() == t_gpu.count(), "blob combine_or level=%u bookmarks=%d", level, bookmarks);
         }
     }
+#ifdef BM64ADDR
+    check_past_2_32(ctx, rng);
+#endif
     std::printf("%s: %d checks, %d failed\n", g_fail ? "FAILED" : "OK", g_checks, g_fail);
     return g_fail ? 1 : 0;
 }

@@ -78,17 +78,19 @@ static void gpu_search(bm::b200::scanner<SV>& sc, int pred, int64_t a, int64_t b
     }
 }
 
+// few = true: four of the search values and no batched forms (the vectors past 2^32, where every search spans 65 539 columns)
 template<class SV>
-static void check_vector(bm::b200::context& ctx, const SV& sv, const char* what, int64_t lo, int64_t hi)
+static void check_vector(bm::b200::context& ctx, const SV& sv, const char* what, int64_t lo, int64_t hi, bool few = false)
 {
     const int64_t i32min = std::numeric_limits<int32_t>::min(), i32max = std::numeric_limits<int32_t>::max();
     bm::sparse_vector_scanner<SV> ref_sc;
     bm::b200::scanner<SV> sc(ctx, sv);
-    const int64_t vals[][2] = {{0, 0}, {-1, 1}, {-2, -1}, {1, -2}, {lo, hi}, {hi, lo}, {lo - 1, lo + 1}, {hi + 1, hi + 9},
-                               {-3, 3}, {7, 7}, {i32min, i32max}, {i32max, i32min}, {i32min + 1, -i32max}};
+    const int64_t vals[][2] = {{0, 0}, {lo, hi}, {-9, 9}, {i32min, i32max}, {-1, 1}, {-2, -1}, {1, -2}, {hi, lo}, {lo - 1, lo + 1},
+                               {hi + 1, hi + 9}, {-3, 3}, {7, 7}, {i32max, i32min}, {i32min + 1, -i32max}};
     auto in_i32 = [&](int64_t x) { return x < i32min ? i32min : x > i32max ? i32max : x; };   // see the file comment
     for (int pred = BMB200_SCAN_EQ; pred <= BMB200_SCAN_RANGE; ++pred) {
-        for (const auto& vv : vals) {
+        for (size_t q = 0; q < (few ? 4u : sizeof(vals) / sizeof(vals[0])); ++q) {
+            const auto& vv = vals[q];
             const int64_t v[2] = {in_i32(vv[0]), in_i32(vv[1])};
             bvect r, g;
             ref_search(ref_sc, sv, pred, v[0], v[1], r);
@@ -96,6 +98,7 @@ static void check_vector(bm::b200::context& ctx, const SV& sv, const char* what,
             CHECK(r.compare(g) == 0 && r.count() == g.count(), "%s pred=%d value=%lld/%lld: count ref %llu gpu %llu", what, pred,
                   (long long)v[0], (long long)v[1], (unsigned long long)r.count(), (unsigned long long)g.count());
         }
+        if (few) continue;
         // batched and count-only forms: two's-complement int64 values in the uint64_t slots
         std::vector<int64_t> sv64 = pred == BMB200_SCAN_RANGE ? std::vector<int64_t>{-2, 40, 300, -10, 0, 0, i32min, -1}
                                                                 : std::vector<int64_t>{0, -3, 77, i32min, -1, i32max};
@@ -125,6 +128,13 @@ static void check_vector(bm::b200::context& ctx, const SV& sv, const char* what,
     }
 }
 
+#ifdef BM64ADDR
+// the reference's signed searches are several times slower in a BM64ADDR build: the vectors below get the short value list there
+static const bool few64 = true;
+#else
+static const bool few64 = false;
+#endif
+
 template<class V>
 static void run_type(bm::b200::context& ctx, std::mt19937_64& rng, const char* tname)
 {
@@ -140,23 +150,54 @@ static void run_type(bm::b200::context& ctx, std::mt19937_64& rng, const char* t
             fill(sv, rng, cs.n, nullable != 0, cs.lo, cs.hi);
             std::snprintf(what, sizeof(what), "%s n=%llu [%lld,%lld] nullable=%d", tname, (unsigned long long)cs.n,
                           (long long)cs.lo, (long long)cs.hi, nullable);
-            check_vector(ctx, sv, what, cs.lo, cs.hi);
+            check_vector(ctx, sv, what, cs.lo, cs.hi, few64);
             if (nullable) {
                 rsc_vect rsc;
                 rsc.load_from(sv);
                 rsc.sync();
                 std::snprintf(what, sizeof(what), "rsc<%s> n=%llu [%lld,%lld]", tname, (unsigned long long)cs.n, (long long)cs.lo,
                               (long long)cs.hi);
-                check_vector(ctx, rsc, what, cs.lo, cs.hi);
+                check_vector(ctx, rsc, what, cs.lo, cs.hi, few64);
             }
         }
     }
 }
 
+#ifdef BM64ADDR
+// ---- BM64ADDR: a nullable sparse_vector<int64_t> and its rsc_sparse_vector of more than 2^32 elements, whose stored elements sit
+// on both sides of 2^32 (columns 65535 / 65536).  test_cxx_binding covers a plain (not nullable) vector past 2^32 ----
+static void check_past_2_32(bm::b200::context& ctx, std::mt19937_64& rng)
+{
+    typedef bm::sparse_vector<int64_t, bvect> svect;
+    typedef bm::rsc_sparse_vector<int64_t, svect> rsc_vect;
+    const uint64_t B = 65536u, G = uint64_t(1) << 32, n = G + 2 * B + 321;
+    svect sv(bm::use_null);
+    sv.resize((svect::size_type)n);
+    std::uniform_int_distribution<int64_t> val(-700, 700);
+    for (uint64_t i = G - 2 * B + 3; i < n; ++i) {
+        if (rng() % 4 == 0) continue;
+        int64_t x = val(rng);
+        if ((i >> 16) == 65536) x = ((i >> 10) & 1u) ? -9 : 9;                                    // runs in the first column past 2^32
+        else if (i % 991 == 0) x = std::numeric_limits<int64_t>::min();
+        sv.set((svect::size_type)i, x);
+    }
+    for (uint64_t i = 0; i < 3000; ++i) sv.set((svect::size_type)(i * 11), int64_t(i % 50) - 25);
+    { BM_DECLARE_TEMP_BLOCK(tb) sv.optimize(tb); }
+    check_vector(ctx, sv, "64: int64_t n=2^32+2*65536+321 nullable", -700, 700, true);
+    rsc_vect rsc;
+    rsc.load_from(sv);
+    rsc.sync();
+    check_vector(ctx, rsc, "64: rsc<int64_t> n=2^32+2*65536+321", -700, 700, true);
+}
+#endif
+
 int main()
 {
     std::mt19937_64 rng(20261016);
     bm::b200::context ctx(0);
+#ifdef BM64ADDR
+    check_past_2_32(ctx, rng);
+#endif
     run_type<int32_t>(ctx, rng, "int32_t");
     run_type<int64_t>(ctx, rng, "int64_t");
     std::printf("test_signed_binding: %d checks, %d failed\n", g_checks, g_fail);

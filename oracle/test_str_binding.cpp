@@ -92,11 +92,38 @@ static void check_vector(bm::b200::context& ctx, const str_svect& sv, const char
     }
 }
 
+#ifdef BM64ADDR
+// ---- BM64ADDR: a str_sparse_vector of more than 2^32 elements.  set(idx, str) places elements past 2^32 without visiting the
+// ones below, so only columns 65534..65538 and a few near 0 hold strings.  Not remap()ped: remap() reads every element once
+// through a const_iterator (calc_octet_stat), 2^32 of them here ----
+static void check_past_2_32(bm::b200::context& ctx, std::mt19937_64& rng, const std::vector<std::string>& dict)
+{
+    const uint64_t B = 65536u, G = uint64_t(1) << 32;
+    std::uniform_int_distribution<size_t> pick(0, dict.size() - 1);
+    for (int nullable = 0; nullable < 2; ++nullable) {
+        str_svect sv(nullable ? bm::use_null : bm::no_null);
+        for (uint64_t i = 0; i < 500; ++i) sv.set((str_svect::size_type)(i * 3), dict[pick(rng)].c_str());
+        for (uint64_t i = G - 2 * B + 9; i < G + 2 * B + 123; ++i) {
+            if (nullable && rng() % 5 == 0) continue;
+            if ((i >> 16) == 65536) sv.set((str_svect::size_type)i, dict[((i >> 12) & 1u)].c_str());     // runs past 2^32
+            else sv.set((str_svect::size_type)i, dict[pick(rng)].c_str());
+        }
+        { BM_DECLARE_TEMP_BLOCK(tb) sv.optimize(tb); }
+        std::vector<std::string> q = {"a", "ab", "x", "zzzzzzzzzzzzzz", dict[0], dict[1], dict[2].substr(0, 2)};
+        for (int k = 0; k < 6; ++k) q.push_back(dict[(size_t)k * 11 % dict.size()]);
+        check_vector(ctx, sv, nullable ? "64: n=2^32+2*65536+123 nullable" : "64: n=2^32+2*65536+123", q);
+    }
+}
+#endif
+
 int main()
 {
     std::mt19937_64 rng(20261017);
     bm::b200::context ctx(0);
     const std::vector<std::string> dict = words(rng, 300);
+#ifdef BM64ADDR
+    check_past_2_32(ctx, rng, dict);
+#endif
     const uint64_t sizes[] = {3u * 65536u + 123u, 1000u, 0u};
     char what[96];
     for (uint64_t n : sizes)
