@@ -5,12 +5,12 @@ host-side mirror of the reference operator surface (aggregator.py, scanner.py, h
 There is no CPU fallback: importing works anywhere, computing needs libbmb200.so and an H100.
 """
 from .capi import (BLK_BIT, BLK_FULL, BLK_GAP, BLK_NULL, F_COUNT_ONLY, F_OPT_COMPRESS, F_OPT_NONE, F_OR_TARGET, F_SIGNED, F_STR_PREFIX,
-                   OP_AND,
+                   F_FLOAT, OP_AND,
                    OP_AND_SUB, OP_OR, OP_XOR, OP_SHIFT_R_AND, BMB200Error, Context, DeviceResult, DeviceRS, DeviceSet,
                    aggregate, aggregate_batch, aggregate_host, default_context, scan, scan_str, rank_compress, rank_decompress,
-                   SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT, SCAN_RANGE, NO_UNIVERSE)
+                   SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT, SCAN_RANGE, SCAN_RANGE_OPEN, NO_UNIVERSE)
 from .hostfmt import BVector, PackedSet, result_to_bvector
-from .scanner import RscSparseVector, SparseVector, SparseVectorScanner, StrSparseVector
+from .scanner import RscSparseVector, SparseVector, SparseVectorFloat, SparseVectorScanner, StrSparseVector
 from .aggregator import (OPT_COMPRESS, OPT_NONE, Aggregator, Pipeline, RSIndex, bit_and, bit_or, bit_or_and, bit_sub, bit_xor, merge,
                          build_rs_index, count_and, count_or, count_sub, count_xor)
 

@@ -25,6 +25,7 @@ OP_OR, OP_AND, OP_AND_SUB, OP_XOR, OP_SHIFT_R_AND = 0, 1, 2, 3, 4
 F_COUNT_ONLY, F_OPT_NONE, F_OPT_COMPRESS, F_OR_TARGET = 1, 0, 2, 4
 F_SIGNED = 8                  # bmb200_scan: s2u planes (plane0 = sign plane), int64 search values
 F_STR_PREFIX = 16             # bmb200_scan_str: compare the first strlen(s) bytes (find_eq_str_prefix)
+F_FLOAT = 32                  # bmb200_scan: sign + 31-bit magnitude planes of float elements, float32 search values
 STR_MAX_PLANES = 2048         # bmb200_scan_str: n_planes limit (strings of up to 256 bytes)
 
 # every symbol include/bmb200.h declares (checked by tests/test_cabi_symbols.py)
@@ -106,6 +107,7 @@ class ScanStrArgsC(C.Structure):
 
 
 SCAN_EQ, SCAN_GT, SCAN_GE, SCAN_LT, SCAN_LE, SCAN_RANGE = range(6)
+SCAN_RANGE_OPEN = 6           # lo < element < hi (find_range_float_unbounded); F_FLOAT only
 NO_UNIVERSE = 0xFFFFFFFF
 
 
@@ -556,15 +558,19 @@ def aggregate_batch(ctx: Context, dset: DeviceSet, op: int, groups, flags: int =
 def scan(ctx: Context, dset: DeviceSet, pred: int, values, plane0: int, n_planes: int, universe: int = NO_UNIVERSE,
          flags: int = 0, nb_from: int = 0, nb_to: int = 0, result: DeviceResult | None = None) -> DeviceResult:
     """bmb200_scan: bit-sliced comparison of the sparse vector whose plane j is set vector plane0 + j against every search
-    value (SCAN_RANGE: rows of (lo, hi)); the result has n_values * n_cols columns, value-major.  With F_SIGNED in flags
-    the values are signed (int64) and plane0 is the sign plane of s2u-encoded elements."""
-    if int(flags) & F_SIGNED:
+    value (SCAN_RANGE / SCAN_RANGE_OPEN: rows of (lo, hi)); the result has n_values * n_cols columns, value-major.  With
+    F_SIGNED in flags the values are signed (int64) and plane0 is the sign plane of s2u-encoded elements; with F_FLOAT they
+    are float32 (their bits are passed, so NaN payloads and -0 keep their meaning) and plane0 is the sign plane of a float vector."""
+    if int(flags) & F_FLOAT:
+        vals = np.ascontiguousarray(np.asarray(values, np.float32)).view(np.uint32).astype(np.uint64)
+    elif int(flags) & F_SIGNED:
         vals = np.ascontiguousarray(np.asarray(values, np.int64).view(np.uint64))
     else:
         vals = np.ascontiguousarray(values, dtype=np.uint64)
-    nv = vals.shape[0] if pred == SCAN_RANGE else vals.size
-    if pred == SCAN_RANGE and (vals.ndim != 2 or vals.shape[1] != 2):
-        raise ValueError("SCAN_RANGE takes an array of (lo, hi) rows")
+    two = pred in (SCAN_RANGE, SCAN_RANGE_OPEN)
+    nv = vals.shape[0] if two else vals.size
+    if two and (vals.ndim != 2 or vals.shape[1] != 2):
+        raise ValueError("SCAN_RANGE / SCAN_RANGE_OPEN take an array of (lo, hi) rows")
     args = ScanArgsC(int(plane0), int(n_planes), int(universe), int(pred), int(flags), ptr(vals), int(nv), int(nb_from), int(nb_to))
     res = result if result is not None else DeviceResult(ctx)
     ctx.check(lib().bmb200_scan(ctx._h, dset._h, C.byref(args), C.byref(res._h)), "scan")

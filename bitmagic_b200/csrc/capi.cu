@@ -1554,7 +1554,14 @@ int bmb200_binop(bmb200_ctx* ctx, const bmb200_set* set, int op, uint32_t va, ui
 int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* a, bmb200_result** inout)
 {
     if (!ctx || !set || !a || !inout || set->ctx != ctx || !a->values || !a->n_values) return BMB200_ERR_BADARG;
-    if (a->pred < BMB200_SCAN_EQ || a->pred > BMB200_SCAN_RANGE || !a->n_planes || a->n_planes > 64u) return BMB200_ERR_BADARG;
+    if (a->pred < BMB200_SCAN_EQ || a->pred > BMB200_SCAN_RANGE_OPEN || !a->n_planes || a->n_planes > 64u) return BMB200_ERR_BADARG;
+    const bool fl = (a->flags & BMB200_F_FLOAT) != 0;
+    const bool two = a->pred == BMB200_SCAN_RANGE || a->pred == BMB200_SCAN_RANGE_OPEN;   // two value slots per search
+    if (fl && ((a->flags & BMB200_F_SIGNED) || a->pred == BMB200_SCAN_EQ || a->n_planes > 32u)) return BMB200_ERR_BADARG;
+    if (a->pred == BMB200_SCAN_RANGE_OPEN && !fl) return BMB200_ERR_BADARG;
+    if (fl)
+        for (size_t k = 0; k < (size_t)a->n_values * (two ? 2 : 1); ++k)
+            if (a->values[k] >> 32) return BMB200_ERR_BADARG;
     if ((uint64_t)a->plane0 + a->n_planes > set->v.n_vec) return BMB200_ERR_RANGE;
     if (a->universe != 0xffffffffu && a->universe >= set->v.n_vec) return BMB200_ERR_RANGE;
     const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
@@ -1580,7 +1587,7 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
     r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
 
     // search values -> device through the (pinned) group staging buffer, 2 words per value
-    const size_t nvals = (size_t)nv * (a->pred == BMB200_SCAN_RANGE ? 2 : 1);
+    const size_t nvals = (size_t)nv * (two ? 2 : 1);
     int rc = stage_group(ctx, reinterpret_cast<const uint32_t*>(a->values), 2 * nvals, nullptr, 0, false);
     if (rc) return bail(rc);
     cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
@@ -1592,20 +1599,24 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
     sp.out.n_groups = nv;
     sp.plane0 = a->plane0; sp.n_planes = a->n_planes; sp.universe = a->universe; sp.pred = (uint32_t)a->pred;
     sp.values = reinterpret_cast<const uint64_t*>(ctx->d_group);
-    // values per pass: find_eq keeps one state per value (4 values share a pass), the inequalities two (2 values), RANGE four (2 values);
-    // single searches use the narrow kernels
-    const int mode = a->pred == BMB200_SCAN_EQ ? 0 : a->pred == BMB200_SCAN_RANGE ? 2 : 1;
+    // values per pass: find_eq keeps one state per value (4 values share a pass), the inequalities two (2 values), RANGE and
+    // RANGE_OPEN four (2 values); single searches use the narrow kernels
+    const int mode = a->pred == BMB200_SCAN_EQ ? 0 : two ? 2 : 1;
     const uint32_t vg = nv == 1 ? 1u : (mode == 0 && nv >= 4 ? 4u : 2u);
     const uint64_t items = (uint64_t)cols * ((nv + vg - 1) / vg);
     uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
     if (grid > items) grid = (uint32_t)items;
-    // BMB200_F_SIGNED selects the signed instantiations (s2u planes, int64 values) with the same launch shapes
+    // BMB200_F_SIGNED selects the signed instantiations (s2u planes, int64 values), BMB200_F_FLOAT the float ones (sign +
+    // magnitude planes, float bits; no find_eq, so MODE 1 / 2 only), with the same launch shapes
     #define BMB200_SCAN_LAUNCH(VG, MODE) \
-        do { if (a->flags & BMB200_F_SIGNED) scan_kernel<VG, MODE, true><<<grid, kAggThreads, 0, ctx->stream>>>(sp); \
+        do { if (a->flags & BMB200_F_SIGNED) scan_kernel<VG, MODE, kEncS2u><<<grid, kAggThreads, 0, ctx->stream>>>(sp); \
              else scan_kernel<VG, MODE><<<grid, kAggThreads, 0, ctx->stream>>>(sp); } while (0)
+    #define BMB200_SCAN_LAUNCH_F(VG, MODE) \
+        do { if (fl) scan_kernel<VG, MODE, kEncFloat><<<grid, kAggThreads, 0, ctx->stream>>>(sp); else BMB200_SCAN_LAUNCH(VG, MODE); } while (0)
     if (mode == 0)      { if (vg == 4) BMB200_SCAN_LAUNCH(4, 0); else if (vg == 2) BMB200_SCAN_LAUNCH(2, 0); else BMB200_SCAN_LAUNCH(1, 0); }
-    else if (mode == 1) { if (vg == 2) BMB200_SCAN_LAUNCH(2, 1); else BMB200_SCAN_LAUNCH(1, 1); }
-    else                { if (vg == 2) BMB200_SCAN_LAUNCH(2, 2); else BMB200_SCAN_LAUNCH(1, 2); }
+    else if (mode == 1) { if (vg == 2) BMB200_SCAN_LAUNCH_F(2, 1); else BMB200_SCAN_LAUNCH_F(1, 1); }
+    else                { if (vg == 2) BMB200_SCAN_LAUNCH_F(2, 2); else BMB200_SCAN_LAUNCH_F(1, 2); }
+    #undef BMB200_SCAN_LAUNCH_F
     #undef BMB200_SCAN_LAUNCH
     if ((rc = after_launch(ctx))) return bail(rc);
     *inout = r;

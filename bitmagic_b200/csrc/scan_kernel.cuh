@@ -1,6 +1,6 @@
 // scan_kernel.cuh -- bit-sliced comparison scan over the planes of a sparse vector (sm_90a).
 //
-// Replaces the reference's sparse_vector_scanner<SV> searches for unsigned and signed sparse vectors
+// Replaces the reference's sparse_vector_scanner<SV> searches for unsigned, signed and float sparse vectors
 //   find_eq   src/bmsparsevec_algo.h:4360-4395 (prepare_and_sub_aggregator :2593-2632 + aggregator::combine_and_sub)
 //   find_gt / find_ge / find_lt / find_le / find_range   src/bmsparsevec_algo.h:1135-1182 (find_gt_horizontal & co.)
 // which the reference builds out of many aggregator / bvector passes over the planes.  Here ONE pass over the
@@ -21,7 +21,7 @@
 // 8 KB shared mask (block-wide run scatter), bit planes stream through 128-bit loads, four planes in flight.
 // The result goes through the same epilogue as the aggregation kernel (popcount, digest, run count, kind, bit->GAP).
 //
-// Signed vectors (SIGNED = true; bm::sparse_vector<int32_t / int64_t>, src/bmbmatrix.h:2536-2569) store u = s2u(x):
+// Signed vectors (ENC = kEncS2u; bm::sparse_vector<int32_t / int64_t>, src/bmbmatrix.h:2536-2569) store u = s2u(x):
 // x >= 0 -> x << 1, x < 0 -> (-(x+1)) << 1 | 1, so plane 0 is the sign plane S and planes 1..n-1 hold the magnitude m
 // (a negative element is -(m+1)).  The reference answers a signed inequality with several whole-vector passes
 // (find_gt_horizontal_s, src/bmsparsevec_algo.h:3032-3219); here it is the same single pass:
@@ -35,6 +35,19 @@
 // find_eq (MODE 0) needs no sign combination: it walks all n planes against s2u(v), which is the exact equality of the
 // stored codes and keeps the EQ-only kernel's register footprint (no S, no per-value sign).  RANGE swaps reversed bounds by
 // signed order when the values are staged.
+//
+// Float vectors (ENC = kEncFloat; bm::sparse_vector_float<sparse_vector<unsigned>>, src/bmsparsevec_float.h) keep a float's
+// sign bit in signs_, its 8 exponent bits in exponents_ and its 23 mantissa bits in mantissas_.  Every float search of the
+// reference (find_gt_float & co., src/bmsparsevec_algo.h:3692-4009, 4-6 whole-vector passes each) is a comparison in the
+// IEEE sign-magnitude total order of the raw bits b: key(b) = sign ? ~b : b | 0x80000000 (-0 < +0, a positive NaN above +inf,
+// a negative NaN below -inf, payloads ordered by their bits).  That is the signed walk above, unchanged:
+//   * the planes are [signs_, mantissa 0..22, exponent 0..7], so plane 1 + k is bit k of the magnitude b & 0x7fffffff;
+//   * the search value is staged as ((b & 0x7fffffff) << 1) | (b >> 31): magnitude in bits 1.., sign in bit 0 -- the same
+//     shape as s2u, and signed_combine gives exactly the key() order (negatives by falling magnitude, -0 below +0);
+//   * RANGE and RANGE_OPEN swap their bounds when a > b as IEEE floats (find_range_float :3819, :3846: a NaN bound never
+//     swaps, +0 / -0 compare equal), decided with integer logic on the bits so no flush-to-zero mode can change it;
+//   * RANGE_OPEN (find_range_float_unbounded) is gt(a) & lt(b) = GT_a & U & ~(GT_b | EQ_b), two state pairs like RANGE.
+// The float path has no find_eq (the reference has none) and so only the MODE 1 / 2 instantiations.
 #pragma once
 #include "gap_expand.cuh"
 
@@ -43,10 +56,10 @@ namespace bmb200 {
 struct ScanParams {
     AggParams out;             // set view + result buffers + work counter (group / goff unused; n_groups = n_values)
     uint32_t  plane0;          // plane j (bit j of the value) = set vector plane0 + j
-    uint32_t  n_planes;        // <= 64
+    uint32_t  n_planes;        // <= 64 (float: <= 32)
     uint32_t  universe;        // set vector holding the searchable index range (size mask / NOT-NULL plane); 0xffffffff = everything
     uint32_t  pred;            // BMB200_SCAN_*
-    const uint64_t* values;    // device: n_values entries (RANGE: 2 * n_values, lo then hi of each range)
+    const uint64_t* values;    // device: n_values entries (RANGE / RANGE_OPEN: 2 * n_values, lo then hi of each range)
 };
 
 constexpr int kScanBatch = 4;  // planes whose loads are issued together
@@ -66,6 +79,21 @@ __device__ __forceinline__ uint64_t s2u(uint64_t v)
     return (int64_t)v >= 0 ? v << 1 : ((~v) << 1) | 1ull;
 }
 
+// a float's 32 bits staged for the signed walk: magnitude (b & 0x7fffffff) in bits 1..31, sign in bit 0
+__device__ __forceinline__ uint64_t f2u(uint64_t b)
+{
+    return ((b & 0x7fffffffull) << 1) | ((b >> 31) & 1ull);
+}
+
+// a > b for the IEEE floats with bits a, b (the C++ comparison find_range_float swaps on), in integer logic: false when either
+// is a NaN or both are zeros, else the key() order of the bits
+__device__ __forceinline__ bool float_gt(uint32_t a, uint32_t b)
+{
+    if ((a & 0x7fffffffu) > 0x7f800000u || (b & 0x7fffffffu) > 0x7f800000u || !((a | b) & 0x7fffffffu)) return false;
+    const uint32_t ka = (a >> 31) ? ~a : a | 0x80000000u, kb = (b >> 31) ? ~b : b | 0x80000000u;
+    return ka > kb;
+}
+
 // (EQm, GTm) of the magnitude walk -> (EQ, GT) of the signed comparison, S = sign plane, neg = the value is negative
 __device__ __forceinline__ void signed_combine(uint4& e, uint4& t, const uint4& U, const uint4& S, bool neg)
 {
@@ -81,11 +109,13 @@ __device__ __forceinline__ void signed_combine(uint4& e, uint4& t, const uint4& 
 // VG search values share one pass over the planes of a column (their states live side by side in registers), so plane loads
 // and GAP expansions are paid once per VG searches; RANGE keeps two state pairs per value and therefore groups fewer values.
 // MODE 0: find_eq only (no GT state), 1: one (EQ, GT) pair per value, 2: RANGE (two pairs per value)
-// SIGNED: s2u-encoded elements, int64 search values (see the file comment)
-template <int VG, int MODE, bool SIGNED = false>
+// ENC: how elements and search values are encoded (see the file comment)
+enum ScanEnc { kEncUnsigned = 0, kEncS2u = 1, kEncFloat = 2 };
+template <int VG, int MODE, int ENC = kEncUnsigned>
 __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const ScanParams sp)
 {
     constexpr bool RANGE = (MODE == 2), EQ_ONLY = (MODE == 0);
+    constexpr bool SIGNED = (ENC != kEncUnsigned);                          // s2u and float elements take the signed walk
     constexpr int kLowPlane = (SIGNED && !EQ_ONLY) ? 1 : 0;                  // the signed inequalities leave the sign plane out of the walk
     constexpr int kStateRegs = VG * (EQ_ONLY ? 4 : RANGE ? 16 : 8);
     constexpr int kBatch = kStateRegs > 16 ? 2 : kScanBatch;                // planes in flight: bounded by the register budget
@@ -121,7 +151,10 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const Sca
         if (tid < VG) {
             const uint32_t vi = min(v0 + (uint32_t)tid, p.n_groups - 1u);         // a short last group repeats its last value
             uint64_t a = sp.values[RANGE ? 2u * vi : vi], b = RANGE ? sp.values[2u * vi + 1u] : 0ull;
-            if constexpr (SIGNED) {
+            if constexpr (ENC == kEncFloat) {
+                if (RANGE && float_gt((uint32_t)a, (uint32_t)b)) { const uint64_t t = a; a = b; b = t; }   // IEEE order, :3819,3846
+                a = f2u(a); b = f2u(b);
+            } else if constexpr (SIGNED) {
                 if (RANGE && (int64_t)b < (int64_t)a) { const uint64_t t = a; a = b; b = t; }   // signed order, :2871-2872
                 a = s2u(a); b = s2u(b);
             } else if (RANGE && b < a) { const uint64_t t = a; a = b; b = t; }    // find_range swaps reversed bounds, :2871-2872
@@ -224,9 +257,13 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const Sca
             case BMB200_SCAN_GE: R = make_uint4(t.x | e.x, t.y | e.y, t.z | e.z, t.w | e.w); break;
             case BMB200_SCAN_LT: R = make_uint4(U.x & ~(t.x | e.x), U.y & ~(t.y | e.y), U.z & ~(t.z | e.z), U.w & ~(t.w | e.w)); break;
             case BMB200_SCAN_LE: R = make_uint4(U.x & ~t.x, U.y & ~t.y, U.z & ~t.z, U.w & ~t.w); break;
-            default: {           // RANGE: ge(a) & le(b)
+            default: {           // RANGE: ge(a) & le(b); RANGE_OPEN (float only): gt(a) & lt(b)
                 const uint4 tb = gtB[RANGE ? g : 0];
-                R = make_uint4((t.x | e.x) & U.x & ~tb.x, (t.y | e.y) & U.y & ~tb.y, (t.z | e.z) & U.z & ~tb.z, (t.w | e.w) & U.w & ~tb.w);
+                if (ENC == kEncFloat && sp.pred == BMB200_SCAN_RANGE_OPEN) {
+                    const uint4 eb = eqB[RANGE ? g : 0];
+                    R = make_uint4(t.x & U.x & ~(tb.x | eb.x), t.y & U.y & ~(tb.y | eb.y), t.z & U.z & ~(tb.z | eb.z), t.w & U.w & ~(tb.w | eb.w));
+                } else
+                    R = make_uint4((t.x | e.x) & U.x & ~tb.x, (t.y | e.y) & U.y & ~tb.y, (t.z | e.z) & U.z & ~tb.z, (t.w | e.w) & U.w & ~tb.w);
                 break; }
             }
             if (g) __syncthreads();                          // the epilogue scratch (K[0]) of the previous value is still being read

@@ -22,6 +22,10 @@
 // byte k) and its universe; find_eq_str / find_eq_str_prefix / the batched string searches are bmb200_scan_str launches
 // (csrc/str_scan_kernel.cuh).  A remapped vector's queries are translated on the host (remap_tosv) and only their codes go to
 // the device.  The numeric searches do not compile for a string vector.
+// A float vector (bm::sparse_vector_float<sparse_vector<unsigned>>, src/bmsparsevec_float.h; detected like the reference's
+// scanner does, through SV::sparse_vector_u) has a specialization of its own: it uploads signs_, mantissas_.get_slice(0..22) and
+// exponents_.get_slice(0..7) as the planes of one BMB200_F_FLOAT scan and offers the reference's find_gt_float / find_ge_float /
+// find_lt_float / find_le_float / find_range_float / find_range_float_unbounded plus batched and count-only forms.
 // bm::b200::rank_compressor<BV> is the device counterpart of bm::rank_compressor<BV> (src/bmalgo.h:451-644).
 #ifndef BMB200_SCANNER_HPP_INCLUDED
 #define BMB200_SCANNER_HPP_INCLUDED
@@ -30,11 +34,13 @@
 #include "bmsparsevec_algo.h"
 #include "bmb200_aggregator.hpp"
 
+#include <cstring>
 #include <string>
+#include <type_traits>
 
 namespace bm { namespace b200 {
 
-template<class SV>
+template<class SV, class = void>
 class scanner
 {
 public:
@@ -272,6 +278,126 @@ private:
     unsigned n_planes_ = 0;
     uint32_t n_blocks_ = 0;
     uint32_t scan_to_ = 0;             // RSC: compressed columns scanned (0 = every column)
+};
+
+/// bm::b200::scanner for bm::sparse_vector_float<sparse_vector<unsigned>> (src/bmsparsevec_float.h, searches
+/// src/bmsparsevec_algo.h:1299-1352,3692-4009).  The set holds the planes [signs_, mantissas_.get_slice(0..22),
+/// exponents_.get_slice(0..7)] -- plane 1 + k is bit k of the magnitude bits & 0x7fffffff; absent slices are empty vectors and
+/// trailing absent ones are trimmed -- and the universe: the NOT-NULL vector of exponents_ (which mantissas_ shares) for a
+/// nullable vector, else [0, size()).  Every search is one bmb200_scan launch with BMB200_F_FLOAT, comparing in the IEEE
+/// sign-magnitude total order of the bits (-0 < +0, NaNs beyond the infinities) as the reference's float searches do.
+template<class SV>
+class scanner<SV, std::void_t<typename SV::sparse_vector_u>>
+{
+public:
+    typedef typename SV::bvector_type bvector_type;
+    typedef typename SV::value_type value_type;
+    typedef typename bvector_type::size_type size_type;
+    static_assert(!SV::sparse_vector_u::is_compressed(),
+                  "bm::b200::scanner: sparse_vector_float<rsc_sparse_vector<>> is not supported (its signs_ stay in the logical space)");
+
+    scanner(context& c, const SV& sv) : ctx_(c) { bind(sv); }
+    ~scanner() { if (set_) bmb200_set_free(set_); }
+    scanner(const scanner&) = delete; scanner& operator=(const scanner&) = delete;
+
+    /// upload the planes + universe of `sv`
+    void bind(const SV& sv)
+    {
+        if (set_) { bmb200_set_free(set_); set_ = nullptr; }
+        size_ = sv.size();
+        n_planes_ = 32;
+        while (n_planes_ > 1 && !plane(sv, n_planes_ - 1)) --n_planes_;
+        n_blocks_ = detail::column_count(std::max<uint64_t>(detail::size_blocks(size_), 1u), "bm::b200::scanner");
+        if (const bvector_type* nn = sv.exponents_.get_null_bvector()) universe_ = *nn;
+        else { universe_.clear(true); if (size_) universe_.set_range(0, size_ - 1); universe_.optimize(); }
+        const uint32_t n_vec = n_planes_ + 1;
+        std::vector<detail::tree_view<bvector_type>> views(n_vec);
+        std::vector<bmb200_vec_blocks> vb(n_vec);
+        bvector_type empty;
+        for (unsigned j = 0; j < n_vec; ++j) {
+            const bvector_type* bv = j < n_planes_ ? plane(sv, j) : &universe_;
+            views[j].build(bv ? *bv : empty, n_blocks_);
+            vb[j].n_blocks = n_blocks_; vb[j].kind = views[j].kind.data(); vb[j].ptr = views[j].ptr.data();
+        }
+        check(bmb200_set_upload_vectors(ctx_.get(), n_vec, n_blocks_, vb.data(), &set_), "bmb200_set_upload_vectors");
+    }
+
+    void find_gt_float(value_type v, bvector_type& bv_out) { one(BMB200_SCAN_GT, v, v, bv_out); }
+    void find_ge_float(value_type v, bvector_type& bv_out) { one(BMB200_SCAN_GE, v, v, bv_out); }
+    void find_lt_float(value_type v, bvector_type& bv_out) { one(BMB200_SCAN_LT, v, v, bv_out); }
+    void find_le_float(value_type v, bvector_type& bv_out) { one(BMB200_SCAN_LE, v, v, bv_out); }
+    /// from <= element <= to; reversed bounds (from > to as floats) are swapped
+    void find_range_float(value_type from, value_type to, bvector_type& bv_out) { one(BMB200_SCAN_RANGE, from, to, bv_out); }
+    /// from < element < to; reversed bounds are swapped
+    void find_range_float_unbounded(value_type from, value_type to, bvector_type& bv_out) { one(BMB200_SCAN_RANGE_OPEN, from, to, bv_out); }
+
+    /// batched searches: one launch, out[k] replaced by the result of search k.  pred = BMB200_SCAN_GT / GE / LT / LE (one value
+    /// per search) or BMB200_SCAN_RANGE / RANGE_OPEN (from, to pairs: two values per search)
+    void find_batch(int pred, const std::vector<value_type>& values, std::vector<bvector_type>& out)
+    {
+        std::vector<uint64_t> v = slots(values);
+        const size_t nv = two(pred) ? v.size() / 2 : v.size();
+        out.resize(nv);
+        run(pred, v.data(), (uint32_t)nv, out.data(), nullptr);
+    }
+    /// cardinalities only (pipeline agg_opt_only_counts); values as in find_batch
+    void count_batch(int pred, const std::vector<value_type>& values, std::vector<size_type>& counts)
+    {
+        std::vector<uint64_t> v = slots(values);
+        const size_t nv = two(pred) ? v.size() / 2 : v.size();
+        counts.assign(nv, 0);
+        run(pred, v.data(), (uint32_t)nv, nullptr, counts.data());
+    }
+
+private:
+    /// plane j: 0 = signs_, 1..23 = mantissa slice j - 1, 24..31 = exponent slice j - 24 (nullptr when absent)
+    static const bvector_type* plane(const SV& sv, unsigned j)
+    {
+        if (j == 0) return &sv.signs_;
+        return j <= 23 ? sv.mantissas_.get_slice(j - 1) : sv.exponents_.get_slice(j - 24);
+    }
+    static bool two(int pred) { return pred == BMB200_SCAN_RANGE || pred == BMB200_SCAN_RANGE_OPEN; }
+    static uint64_t slot(value_type v) { uint32_t b; std::memcpy(&b, &v, sizeof b); return b; }
+    static std::vector<uint64_t> slots(const std::vector<value_type>& values)
+    {
+        std::vector<uint64_t> v(values.size());
+        for (size_t k = 0; k < values.size(); ++k) v[k] = slot(values[k]);
+        return v;
+    }
+    void one(int pred, value_type a, value_type b, bvector_type& bv_out)
+    {
+        const uint64_t v[2] = {slot(a), slot(b)};
+        run(pred, v, 1, &bv_out, nullptr);
+    }
+    void run(int pred, const uint64_t* values, uint32_t nv, bvector_type* out, size_type* counts)
+    {
+        if (!nv) return;
+        const uint32_t flags = (out ? BMB200_F_OPT_COMPRESS : BMB200_F_COUNT_ONLY) | BMB200_F_FLOAT;
+        bmb200_scan_args a{0u, n_planes_, n_planes_, pred, flags, values, nv, 0u, 0u};
+        bmb200_result* res = nullptr;
+        int rc = bmb200_scan(ctx_.get(), set_, &a, &res);
+        const size_t ncols = (size_t)nv * n_blocks_;
+        std::vector<uint64_t> totals(nv);
+        std::vector<uint8_t> kind(ncols); std::vector<uint64_t> off(ncols); std::vector<uint32_t> bits; std::vector<uint16_t> gaps;
+        if (!rc) rc = bmb200_result_group_totals(res, totals.data(), nv);
+        if (!rc && out) { uint64_t nb = 0, ng = 0; rc = bmb200_result_sizes(res, &nb, &ng);
+                          if (!rc) { bits.resize(nb * BMB200_BLOCK_WORDS); gaps.resize(ng);
+                                     rc = bmb200_result_fetch(res, kind.data(), off.data(), bits.data(), gaps.data()); } }
+        if (res) bmb200_result_free(res);
+        check(rc, "bmb200_scan");
+        for (uint32_t k = 0; k < nv; ++k) {
+            if (counts) counts[k] = (size_type)totals[k];
+            if (out) detail::store_result(out[k], size_, n_blocks_, kind.data() + (size_t)k * n_blocks_, off.data() + (size_t)k * n_blocks_,
+                                          bits.data(), gaps.data());
+        }
+    }
+
+    context& ctx_;
+    bmb200_set* set_ = nullptr;
+    bvector_type universe_;
+    size_type size_ = 0;
+    unsigned n_planes_ = 0;
+    uint32_t n_blocks_ = 0;
 };
 
 /// bm::rank_compressor<BV> (src/bmalgo.h:451-644) on the device: the index vector and the source are uploaded for the call,

@@ -18,6 +18,12 @@ element as ``s2u(x)`` (src/bmbmatrix.h:2536-2569: ``x >= 0 -> x << 1``, ``x < 0 
 sign plane.  Their searches take int64 values and run with ``F_SIGNED``; ``find_zero / find_nonzero`` stay unsigned searches
 for 0 over the same planes, which is what the reference computes for them (an OR of all planes).
 
+Float vectors (``bm::sparse_vector_float<sparse_vector<unsigned>>``, ``SparseVectorFloat``) keep a float's sign bit in
+``signs_``, its exponent in ``exponents_`` and its mantissa in ``mantissas_``.  Their planes are laid out as
+``[signs_, mantissa 0..22, exponent 0..7]`` -- plane 1 + k is bit k of the magnitude ``bits & 0x7fffffff`` -- and their
+searches (``find_gt_float`` & co.) run with ``F_FLOAT`` and float32 values.  They compare in the IEEE sign-magnitude total
+order of the bits (-0 < +0, NaNs beyond the infinities), as the reference's float searches do; there is no float ``find_eq``.
+
 String vectors (``bm::str_sparse_vector<char, ...>``, ``StrSparseVector``) keep bit b of byte k of every element in plane 8k+b;
 ``find_eq_str`` / ``find_eq_str_prefix`` / ``count_eq_str`` run as ``bmb200_scan_str`` (csrc/str_scan_kernel.cuh).  The numeric
 searches raise on a string vector.
@@ -27,7 +33,8 @@ from __future__ import annotations
 import numpy as np
 
 from . import capi
-from .capi import F_COUNT_ONLY, F_OPT_COMPRESS, F_SIGNED, F_STR_PREFIX, SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT, SCAN_RANGE
+from .capi import (F_COUNT_ONLY, F_FLOAT, F_OPT_COMPRESS, F_SIGNED, F_STR_PREFIX, SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT,
+                   SCAN_RANGE, SCAN_RANGE_OPEN)
 from .hostfmt import BLOCK_BITS, BVector, PackedSet, bits_to_words, result_to_bvector
 
 
@@ -83,6 +90,24 @@ class SparseVector:
         bits = np.zeros(nb * BLOCK_BITS, np.uint8)
         bits[:self.size] = 1
         return BVector.from_words(bits_to_words(bits)).optimize()
+
+
+def f2u(values) -> np.ndarray:
+    """float32 values -> their bits as the float planes hold them: magnitude (bits & 0x7fffffff) in bits 1..31, sign in bit 0"""
+    b = np.ascontiguousarray(values, dtype=np.float32).view(np.uint32).astype(np.uint64)
+    return ((b & np.uint64(0x7FFFFFFF)) << np.uint64(1)) | (b >> np.uint64(31))
+
+
+class SparseVectorFloat(SparseVector):
+    """``bm::sparse_vector_float<sparse_vector<unsigned>>`` as the scanner sees it: plane 0 = ``signs_``, planes 1..23 =
+    ``mantissas_.get_slice(0..22)``, planes 24..31 = ``exponents_.get_slice(0..7)``, trailing empty planes trimmed; for a
+    nullable vector the NOT-NULL plane that ``mantissas_`` shares with ``exponents_``."""
+
+    @classmethod
+    def from_values(cls, values, null_mask=None, optimize: bool = True) -> "SparseVectorFloat":
+        """set(i, value) for every non-NULL i (NULL elements and unassigned positions hold no bit) + optimize()"""
+        sv = SparseVector.from_values(f2u(values), null_mask, optimize)
+        return cls(sv.planes, sv.size, sv.not_null)
 
 
 class RscSparseVector:
@@ -181,6 +206,7 @@ class SparseVectorScanner:
         self.sv = sv
         self._rsc = isinstance(sv, RscSparseVector)
         self._str = isinstance(sv, StrSparseVector)
+        self._float = isinstance(sv, SparseVectorFloat)
         vecs = list(sv.planes) + [sv.universe()]
         if self._rsc:
             # one set as wide as the logical space: compressed planes (NULL past their columns), [0, effective_size), NN
@@ -201,15 +227,19 @@ class SparseVectorScanner:
             self._dset.free()
             self._dset = None
 
-    def _run(self, pred, values, count_only=False, signed=None):
-        """signed: compare as signed values (default: the vector's signedness); find_zero / find_nonzero pass False"""
+    def _run(self, pred, values, count_only=False, signed=None, fl=False):
+        """signed: compare as signed values (default: the vector's signedness); find_zero / find_nonzero pass False.
+        fl: a float search (the *_float methods), float32 values"""
         if self._str:
             raise TypeError("numeric searches do not apply to a string vector: use find_eq_str / find_eq_str_prefix")
+        if fl != self._float:
+            raise TypeError("a float vector is searched with the *_float methods" if self._float else "the *_float searches need a SparseVectorFloat")
         signed = self.sv.signed if signed is None else signed
-        single = np.ndim(values) == (1 if pred == SCAN_RANGE else 0)
-        dt = np.int64 if signed else np.uint64
-        vals = np.atleast_2d(np.asarray(values, dt)) if pred == SCAN_RANGE else np.atleast_1d(np.asarray(values, dt))
-        flags = (F_COUNT_ONLY if count_only else F_OPT_COMPRESS) | (F_SIGNED if signed else 0)
+        two = pred in (SCAN_RANGE, SCAN_RANGE_OPEN)
+        single = np.ndim(values) == (1 if two else 0)
+        dt = np.float32 if fl else np.int64 if signed else np.uint64
+        vals = np.atleast_2d(np.asarray(values, dt)) if two else np.atleast_1d(np.asarray(values, dt))
+        flags = (F_COUNT_ONLY if count_only else F_OPT_COMPRESS) | (F_SIGNED if signed else 0) | (F_FLOAT if fl else 0)
         res = capi.scan(self.ctx, self._dset, pred, vals, 0, self.sv.effective_slices(), self._universe, flags, 0, self._scan_to)
         return self._results(res, vals.shape[0], count_only, single)
 
@@ -260,6 +290,23 @@ class SparseVectorScanner:
     def count_gt(self, value):   return self._run(SCAN_GT, value, True)
     def count_range(self, lo, hi=None):
         return self._run(SCAN_RANGE, [lo, hi] if hi is not None else lo, True)
+    # float vectors: float32 values (one, or a list = one launch); ranges as (from, to) or a list of such rows
+    def find_gt_float(self, value):  return self._run(SCAN_GT, value, fl=True)
+    def find_ge_float(self, value):  return self._run(SCAN_GE, value, fl=True)
+    def find_lt_float(self, value):  return self._run(SCAN_LT, value, fl=True)
+    def find_le_float(self, value):  return self._run(SCAN_LE, value, fl=True)
+    def find_range_float(self, lo, hi=None):
+        return self._run(SCAN_RANGE, [lo, hi] if hi is not None else lo, fl=True)
+    def find_range_float_unbounded(self, lo, hi=None):
+        return self._run(SCAN_RANGE_OPEN, [lo, hi] if hi is not None else lo, fl=True)
+    def count_gt_float(self, value): return self._run(SCAN_GT, value, True, fl=True)
+    def count_ge_float(self, value): return self._run(SCAN_GE, value, True, fl=True)
+    def count_lt_float(self, value): return self._run(SCAN_LT, value, True, fl=True)
+    def count_le_float(self, value): return self._run(SCAN_LE, value, True, fl=True)
+    def count_range_float(self, lo, hi=None):
+        return self._run(SCAN_RANGE, [lo, hi] if hi is not None else lo, True, fl=True)
+    def count_range_float_unbounded(self, lo, hi=None):
+        return self._run(SCAN_RANGE_OPEN, [lo, hi] if hi is not None else lo, True, fl=True)
     # string vectors: one query (bytes / str) or a list of them (one launch)
     def find_eq_str(self, s):         return self._run_str(s, False)
     def find_eq_str_prefix(self, s):  return self._run_str(s, True)

@@ -23,6 +23,9 @@
  *   bmb200_set_upload_blobs       <- bm::deserialize / deserializer<BV>::deserialize  src/bmserial.h:4152,5578-6090
  *   bmb200_scan                   <- sparse_vector_scanner::find_eq/find_gt/find_ge/find_lt/find_le/find_range
  *                                                                   src/bmsparsevec_algo.h:1083-1182,2593-2632,4360-4395
+ *   bmb200_scan  BMB200_F_FLOAT   <- sparse_vector_scanner::find_gt_float/find_ge_float/find_lt_float/find_le_float/
+ *                                    find_range_float/find_range_float_unbounded over sparse_vector_float
+ *                                                                   src/bmsparsevec_algo.h:1299-1352,3692-4009
  *   bmb200_scan_str               <- sparse_vector_scanner::find_eq_str / find_eq_str_prefix / find_eq_str(TPipe&) over
  *                                    str_sparse_vector            src/bmsparsevec_algo.h:2546-2588,3263-3436,4579-4651
  *   bmb200_rs_build               <- bvector::build_rs_index       src/bm.h:2531-2660, rs_index src/bmrs.h:688-715
@@ -94,6 +97,8 @@ extern "C" {
 #define BMB200_F_OR_TARGET   4u  /* batch only: also accumulate the union of all group results (pipeline::set_or_target) */
 #define BMB200_F_SIGNED      8u  /* bmb200_scan only: the planes hold s2u-encoded signed elements (plane plane0 = sign plane)
                                   * and values[] are int64_t in two's complement (see bmb200_scan)                         */
+#define BMB200_F_FLOAT      32u  /* bmb200_scan only: the planes hold float elements as sign + 31-bit magnitude (plane plane0 =
+                                  * sign plane) and values[] hold float bits, zero-extended (see bmb200_scan)              */
 
 typedef struct bmb200_ctx    bmb200_ctx;     /* one per process per GPU                      */
 typedef struct bmb200_set    bmb200_set;     /* device-resident column-major set of vectors  */
@@ -339,23 +344,34 @@ int bmb200_result_free(bmb200_result* res);
  * BMB200_F_SIGNED: element x is stored as u = s2u(x) (src/bmbmatrix.h: x >= 0 -> x << 1, x < 0 -> (-(x+1)) << 1 | 1), so
  * plane0 is the sign plane and planes 1..n_planes-1 hold the magnitude; values[] are then int64_t (passed in the uint64_t
  * slots), compared as signed integers, and RANGE swaps reversed bounds by signed order.  find_zero / find_nonzero of a
- * signed vector are the unsigned EQ 0 / GT 0 over the same planes (the reference ORs all planes, sign included). */
+ * signed vector are the unsigned EQ 0 / GT 0 over the same planes (the reference ORs all planes, sign included).
+ * Float vectors (bm::sparse_vector_float<sparse_vector<unsigned>>: signs_, exponents_, mantissas_) are searched with
+ * BMB200_F_FLOAT: plane plane0 is signs_ and plane plane0 + 1 + k is bit k of the 31-bit magnitude b & 0x7fffffff of the
+ * element's bits b -- mantissas_.get_slice(0..22), then exponents_.get_slice(0..7) -- with n_planes 1..32 (trailing absent
+ * planes may be trimmed).  values[] hold float bits, zero-extended.  Every float search compares in the IEEE sign-magnitude
+ * total order key(b) = sign ? ~b : b | 0x80000000 (-0 < +0, NaNs beyond the infinities, payloads by their bits), which is
+ * what the reference's find_*_float compute; RANGE (find_range_float) and RANGE_OPEN (find_range_float_unbounded) swap
+ * their bounds when from > to as C++ floats (a NaN bound never swaps; +0 and -0 do not swap).  BMB200_ERR_BADARG for
+ * BMB200_F_FLOAT with BMB200_F_SIGNED, with BMB200_SCAN_EQ (the reference has no float find_eq), with n_planes > 32 or with
+ * a value slot that has bits above 31, and for BMB200_SCAN_RANGE_OPEN without BMB200_F_FLOAT. */
 #define BMB200_SCAN_EQ     0   /* find_eq    src/bmsparsevec_algo.h:1083  elements == value                    */
 #define BMB200_SCAN_GT     1   /* find_gt    :1135                        elements >  value                    */
 #define BMB200_SCAN_GE     2   /* find_ge    :1144                                                             */
 #define BMB200_SCAN_LT     3   /* find_lt    :1154                                                             */
 #define BMB200_SCAN_LE     4   /* find_le    :1163                                                             */
 #define BMB200_SCAN_RANGE  5   /* find_range :1174  values[2k] <= element <= values[2k+1] (reversed bounds are swapped, :2871) */
+#define BMB200_SCAN_RANGE_OPEN 6 /* find_range_float_unbounded :3841  values[2k] < element < values[2k+1]; BMB200_F_FLOAT only */
 typedef struct bmb200_scan_args {
     uint32_t        plane0;     /* first plane vector inside the set                                          */
-    uint32_t        n_planes;   /* 1..64 (sparse_vector::effective_slices())                                  */
+    uint32_t        n_planes;   /* 1..64 (sparse_vector::effective_slices()); BMB200_F_FLOAT: 1..32           */
     uint32_t        universe;   /* set vector with the searchable indexes: [0, size) for a non-nullable vector,
                                  * the NOT-NULL plane for a nullable one (what finalize_search_result and
                                  * invert_internal apply, :2426,1686); 0xffffffff = every index of the columns */
     int32_t         pred;       /* BMB200_SCAN_*                                                              */
-    uint32_t        flags;      /* BMB200_F_COUNT_ONLY / BMB200_F_OPT_COMPRESS, | BMB200_F_SIGNED              */
-    const uint64_t* values;     /* HOST: n_values search values (RANGE: 2 * n_values, lo then hi);
-                                 * with BMB200_F_SIGNED each is an int64_t in two's complement                */
+    uint32_t        flags;      /* BMB200_F_COUNT_ONLY / BMB200_F_OPT_COMPRESS, | BMB200_F_SIGNED or BMB200_F_FLOAT */
+    const uint64_t* values;     /* HOST: n_values search values (RANGE / RANGE_OPEN: 2 * n_values, lo then hi);
+                                 * with BMB200_F_SIGNED each is an int64_t in two's complement, with
+                                 * BMB200_F_FLOAT the 32 bits of a float, zero-extended                        */
     uint32_t        n_values;
     uint32_t        nb_from;
     uint32_t        nb_to;      /* 0 == n_blocks */
