@@ -45,7 +45,7 @@ SYMBOLS = [
     "bmb200_set_upload_slabs", "bmb200_host_slabs_prefetch", "bmb200_host_slab_alloc", "bmb200_host_slab_free",
     "bmb200_result_fetch_view_async", "bmb200_result_fetch_wait", "bmb200_exchange_mode",
     "bmb200_result_fetch_column", "bmb200_set_run_lists", "bmb200_set_bit_run_lists",
-    "bmb200_rank_decompress", "bmb200_rank_compress", "bmb200_scan_str",
+    "bmb200_rank_decompress", "bmb200_rank_compress", "bmb200_scan_str", "bmb200_set_packed_singles",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
@@ -135,8 +135,8 @@ def lib() -> C.CDLL:
         _lib = C.CDLL(str(LIB_PATH))
         _lib.bmb200_error_msg.restype = C.c_char_p
         _lib.bmb200_error_msg.argtypes = [C.c_int]
-        for name in SYMBOLS:
-            if name != "bmb200_error_msg":
+        for name in SYMBOLS:            # an older build (BMB200_LIB) loads without the entry points it lacks
+            if name != "bmb200_error_msg" and hasattr(_lib, name):
                 getattr(_lib, name).restype = C.c_int
     return _lib
 
@@ -432,6 +432,13 @@ class DeviceSet:
         a, b, n = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
         self.ctx.check(lib().bmb200_set_bit_run_lists(self._h, C.byref(a), C.byref(b), C.byref(n)), "set_bit_run_lists")
         return a.value, b.value, n.value
+
+    def packed_singles_bytes(self) -> tuple[int, int]:
+        """Bytes of the companion's singles as resident and streamed (16-byte word units), of part A and of part B; (0, 0) while
+        none is built."""
+        a, b = C.c_uint64(0), C.c_uint64(0)
+        self.ctx.check(lib().bmb200_set_packed_singles(self._h, C.byref(a), C.byref(b)), "set_packed_singles")
+        return a.value, b.value
 
     def stored_bytes(self) -> int:
         """Algorithmic source bytes: 8192 per bit-block + the 16-byte units of the GAP blocks."""

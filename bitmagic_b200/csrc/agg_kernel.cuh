@@ -302,18 +302,17 @@ __device__ __forceinline__ void flat_quad(uint32_t Ls, const uint4& q)
     if (reach > 32u) flat_quad_tail(Ls, q);
 }
 
-// Singles of the run-list companion (runlist_kernel.cuh): eight u16 bit positions per 128-bit load, one bit each, one atomic per
-// position.  The singles are dealt out by bank, so a warp's atomic is one shared-memory wavefront in a part's full rounds, and a
-// test-first form (`lds32`, then a predicated atomic, as flat_quad's MODE 1) only adds a dependent shared-memory round trip per
-// position: it was 0.9 % slower on C3 (2.202-2.205 against 2.182 ms, H100 80GB HBM3 at 700 W), where L is 12 % alive and less.
-__device__ __forceinline__ void sgl_oct(uint32_t Ls, const uint4& q)
+// Singles of the run-list companion (runlist_kernel.cuh): one word unit per 128-bit load, 23 five-bit offsets inside one word of L
+// OR-ed into one mask, one atomic per unit.  The units are dealt out by bank, so a warp's atomic is one shared-memory wavefront in a
+// part's full rounds.
+__device__ __forceinline__ void sgl_unit(uint32_t Ls, const uint4& q)
 {
     const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+    uint32_t m = 0;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        reds_and(and_or(w[i] >> 3, 0x1ffcu, Ls), ~(1u << (w[i] & 31u)));
-        reds_and(and_or(w[i] >> 19, 0x1ffcu, Ls), ~(1u << ((w[i] >> 16) & 31u)));
-    }
+    for (int f = 0; f < 23; ++f) m |= 1u << ((w[f / 6] >> (5 * (f % 6))) & 31u);
+    const uint32_t word = (q.x >> 30) | ((q.y >> 30) << 2) | ((q.z >> 30) << 4) | ((q.w >> 25) << 6);
+    reds_and(Ls + 4u * word, ~m);
 }
 
 // One slot of the FLAT window (bytes = what the bulk copy delivered, a multiple of 16; src = slot address + lane * 16): every lane eats
@@ -323,7 +322,7 @@ __device__ __forceinline__ void sgl_oct(uint32_t Ls, const uint4& q)
 template <int MODE, bool SGL = false>
 __device__ __forceinline__ void flat_sweep_mode(uint32_t Ls, uint32_t src, uint32_t bytes, uint32_t lane_off)
 {
-    auto eat = [&](const uint4& q) { if (SGL) sgl_oct(Ls, q); else flat_quad<MODE>(Ls, q); };
+    auto eat = [&](const uint4& q) { if (SGL) sgl_unit(Ls, q); else flat_quad<MODE>(Ls, q); };
     uint32_t h = 0;
 #pragma unroll 1
     for (; h + 1024u <= bytes; h += 1024u) {
@@ -1072,11 +1071,11 @@ __global__ void desc_flat_check_kernel(const uint32_t* __restrict__ desc, size_t
 // when no GAP block of the set belongs to the AND group; the kernel then streams each column's singles and long runs in place of its
 // GAP segment: part A only (listed null), or A + B (listed set: then no listed bit-block belongs to the AND group either).
 struct RunLists {
-    const uint64_t* sgl_base;   // [n_blocks+1] 16-byte units of sgl
+    const uint64_t* sgl_base;   // [n_blocks+1] word units of sgl
     const uint64_t* lr_base;    // [n_blocks+1] 16-byte units of lr
     const uint64_t* sgl_mid;    // [n_blocks] end of column nb's part A singles = start of its part B
     const uint64_t* lr_mid;     // [n_blocks] ... long runs
-    const uint16_t* sgl;        // singles: u16 bit positions
+    const uint4* sgl;           // singles: word units (runlist_kernel.cuh)
     const uint32_t* lr;         // long runs: FLAT pairs
     const uint32_t* listed;     // bit i: bit-block i of bit_pool is in part B and not streamed; null = stream part A only
 };
@@ -1135,7 +1134,7 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
                 const uint64_t s0 = rl.sgl_base[nb], l0 = rl.lr_base[nb];
                 const uint64_t s1 = rl.listed ? rl.sgl_base[nb + 1] : rl.sgl_mid[nb], l1 = rl.listed ? rl.lr_base[nb + 1] : rl.lr_mid[nb];
                 gbytes = (uint32_t)((s1 - s0) * 16u); lbytes = (uint32_t)((l1 - l0) * 16u);
-                gsrc = reinterpret_cast<const uint8_t*>(rl.sgl + s0 * 8u); lsrc = reinterpret_cast<const uint8_t*>(rl.lr + l0 * 4u);
+                gsrc = reinterpret_cast<const uint8_t*>(rl.sgl + s0); lsrc = reinterpret_cast<const uint8_t*>(rl.lr + l0 * 4u);
                 if (rl.listed) {        // stage the column's listed flags (bit j = bit-block j) and their running counts for everyone
                     const uint32_t* lw = rl.listed + (b0 >> 5);
                     const uint32_t sh = (uint32_t)b0 & 31u, nw = (nbit + 31u) / 32u;

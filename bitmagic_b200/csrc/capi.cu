@@ -117,11 +117,12 @@ struct bmb200_set {
     int rl_state = 0;                       // 0 not built, 1 built, -1 cannot be built (device memory): calls run without it
     uint32_t rl_calls = 0;                  // qualifying calls seen while not built
     uint64_t *rl_sgl_base = nullptr, *rl_lr_base = nullptr, *rl_sgl_mid = nullptr, *rl_lr_mid = nullptr;
-    uint16_t* rl_sgl = nullptr;
+    uint32_t* rl_sgl = nullptr;             // singles in word units (4 u32 each)
     uint32_t* rl_lr = nullptr;
     uint32_t* rl_listed = nullptr;          // bit i: bit-block i of bit_pool is listed in part B
-    uint64_t rl_sgl_units = 0, rl_lr_units = 0;        // part A
+    uint64_t rl_sgl_units = 0, rl_lr_units = 0;        // part A in the list form (bmb200_set_run_lists)
     uint64_t rl_b_sgl_units = 0, rl_b_lr_units = 0, rl_listed_blocks = 0;   // part B
+    uint64_t rl_sgl_word_units = 0, rl_b_sgl_word_units = 0;               // the singles as stored: word units of A, of B
     std::vector<uint32_t> listed_vecs;      // bit v: vector v holds a listed bit-block in some column (set with the companion)
     size_t cap_desc = 0, cap_base = 0, cap_bit = 0, cap_gap = 0;   // capacities when the arrays came from set_alloc (elements / blocks / units); 0 = not recyclable
 };
@@ -225,6 +226,7 @@ void free_run_lists(bmb200_set* s)
     cudaFree(s->rl_sgl); cudaFree(s->rl_lr); cudaFree(s->rl_listed);
     s->rl_sgl_base = s->rl_lr_base = s->rl_sgl_mid = s->rl_lr_mid = nullptr; s->rl_sgl = nullptr; s->rl_lr = nullptr; s->rl_listed = nullptr;
     s->rl_sgl_units = s->rl_lr_units = s->rl_b_sgl_units = s->rl_b_lr_units = s->rl_listed_blocks = 0;
+    s->rl_sgl_word_units = s->rl_b_sgl_word_units = 0;
     s->listed_vecs.clear();
 }
 
@@ -1335,7 +1337,7 @@ static const std::vector<uint32_t>& gap_vectors(bmb200_ctx* ctx, const bmb200_se
 }
 
 // Builds the run-list companion (runlist_kernel.cuh): count pass (which also lists the sparse bit-blocks), scans, one wait to size
-// the pools, write pass, then which vectors hold a listed block.  On any failure, or when parts A + B would leave less than
+// the pools, write pass into the zeroed singles pool, then which vectors hold a listed block.  On any failure, or when parts A + B would leave less than
 // kRunListMargin of device memory free, the set is marked as having none (rl_state = -1).
 constexpr size_t kRunListMargin = size_t(1) << 30;
 static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
@@ -1343,10 +1345,10 @@ static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
     const uint32_t nb = s->v.n_blocks, M = s->v.n_vec, vwords = (M + 31u) / 32u;
     const size_t lwords = (size_t)(s->n_bit_blocks + 31u) / 32u + 2u;   // + the word the kernel's funnel shift reads past a column
     cudaStream_t st = ctx->stream;
-    uint2* wcnt = nullptr; uint64_t *su = nullptr, *lu = nullptr; unsigned long long* tot = nullptr; uint32_t* lv = nullptr;
-    uint64_t h_tot[5] = {0, 0, 0, 0, 0};
+    uint32_t* wlr = nullptr; uint64_t *su = nullptr, *lu = nullptr; unsigned long long* tot = nullptr; uint32_t* lv = nullptr;
+    uint64_t h_tot[7] = {0, 0, 0, 0, 0, 0, 0};
     std::vector<uint32_t> h_lv(vwords, 0u);
-    bool ok = cudaMalloc((void**)&wcnt, (size_t)nb * kRlCnt * sizeof(uint2)) == cudaSuccess &&
+    bool ok = cudaMalloc((void**)&wlr, (size_t)nb * kRlCnt * 4u) == cudaSuccess &&
               cudaMalloc((void**)&su, (size_t)nb * 8) == cudaSuccess && cudaMalloc((void**)&lu, (size_t)nb * 8) == cudaSuccess &&
               cudaMalloc((void**)&tot, sizeof(h_tot)) == cudaSuccess && cudaMalloc((void**)&lv, vwords * 4u) == cudaSuccess &&
               cudaMalloc((void**)&s->rl_sgl_base, ((size_t)nb + 1) * 8) == cudaSuccess &&
@@ -1356,29 +1358,31 @@ static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
               cudaMemsetAsync(s->rl_listed, 0, lwords * 4u, st) == cudaSuccess && cudaMemsetAsync(tot, 0, sizeof(h_tot), st) == cudaSuccess &&
               cudaMemsetAsync(lv, 0, vwords * 4u, st) == cudaSuccess;
     if (ok) {
-        rl_count_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wcnt, su, lu, s->rl_listed, tot);
+        rl_count_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wlr, su, lu, s->rl_listed, tot);
         scan_u64_kernel<<<1, 1024, 0, st>>>(su, nb, s->rl_sgl_base);
         scan_u64_kernel<<<1, 1024, 0, st>>>(lu, nb, s->rl_lr_base);
         ok = cudaGetLastError() == cudaSuccess && cudaMemcpyAsync(h_tot, tot, sizeof(h_tot), cudaMemcpyDeviceToHost, st) == cudaSuccess &&
              cudaStreamSynchronize(st) == cudaSuccess;
     }
-    const uint64_t sgl_units = h_tot[0] + h_tot[2], lr_units = h_tot[1] + h_tot[3];
+    const uint64_t sgl_units = h_tot[5] + h_tot[6], lr_units = h_tot[1] + h_tot[3];
     size_t free_b = 0, total_b = 0;
     ok = ok && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b >= (sgl_units + lr_units) * 16u + kRunListMargin &&
          cudaMalloc((void**)&s->rl_sgl, std::max<uint64_t>(sgl_units, 1u) * 16u) == cudaSuccess &&
-         cudaMalloc((void**)&s->rl_lr, std::max<uint64_t>(lr_units, 1u) * 16u) == cudaSuccess;
+         cudaMalloc((void**)&s->rl_lr, std::max<uint64_t>(lr_units, 1u) * 16u) == cudaSuccess &&
+         cudaMemsetAsync(s->rl_sgl, 0, sgl_units * 16u, st) == cudaSuccess;
     if (ok) {
-        rl_write_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wcnt, s->rl_sgl_base, s->rl_lr_base, s->rl_listed, s->rl_sgl, s->rl_lr,
+        rl_write_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wlr, s->rl_sgl_base, s->rl_lr_base, s->rl_listed, s->rl_sgl, s->rl_lr,
                                                    s->rl_sgl_mid, s->rl_lr_mid);
         const dim3 grid((M + 255u) / 256u, std::min(nb, 256u));
         if (h_tot[4]) listed_vectors_kernel<<<grid, 256, 0, st>>>(s->v.desc, s->v.bit_base, s->rl_listed, M, nb, lv);
         ok = cudaGetLastError() == cudaSuccess && cudaMemcpyAsync(h_lv.data(), lv, vwords * 4u, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
              cudaStreamSynchronize(st) == cudaSuccess;
     }
-    cudaFree(wcnt); cudaFree(su); cudaFree(lu); cudaFree(tot); cudaFree(lv);
+    cudaFree(wlr); cudaFree(su); cudaFree(lu); cudaFree(tot); cudaFree(lv);
     if (!ok) { cudaGetLastError(); free_run_lists(s); s->rl_state = -1; return false; }
     s->rl_sgl_units = h_tot[0]; s->rl_lr_units = h_tot[1];
     s->rl_b_sgl_units = h_tot[2]; s->rl_b_lr_units = h_tot[3]; s->rl_listed_blocks = h_tot[4];
+    s->rl_sgl_word_units = h_tot[5]; s->rl_b_sgl_word_units = h_tot[6];
     s->listed_vecs.swap(h_lv); s->rl_state = 1;
     return true;
 }
@@ -1398,7 +1402,7 @@ static bool use_run_lists(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_b
     bool part_b = s->rl_listed_blocks != 0;
     for (uint32_t k = a->offsets[0]; part_b && k < a->offsets[1]; ++k)
         if ((s->listed_vecs[a->members[k] >> 5] >> (a->members[k] & 31u)) & 1u) part_b = false;
-    *rl = RunLists{s->rl_sgl_base, s->rl_lr_base, s->rl_sgl_mid, s->rl_lr_mid, s->rl_sgl, s->rl_lr, part_b ? s->rl_listed : nullptr};
+    *rl = RunLists{s->rl_sgl_base, s->rl_lr_base, s->rl_sgl_mid, s->rl_lr_mid, reinterpret_cast<const uint4*>(s->rl_sgl), s->rl_lr, part_b ? s->rl_listed : nullptr};
     return true;
 }
 
@@ -1413,6 +1417,13 @@ int bmb200_set_bit_run_lists(const bmb200_set* s, uint64_t* sgl_bytes, uint64_t*
 {
     if (!s || !sgl_bytes || !lr_bytes || !listed_blocks) return BMB200_ERR_BADARG;
     *sgl_bytes = s->rl_b_sgl_units * 16u; *lr_bytes = s->rl_b_lr_units * 16u; *listed_blocks = s->rl_listed_blocks;
+    return BMB200_OK;
+}
+
+int bmb200_set_packed_singles(const bmb200_set* s, uint64_t* a_bytes, uint64_t* b_bytes)
+{
+    if (!s || !a_bytes || !b_bytes) return BMB200_ERR_BADARG;
+    *a_bytes = s->rl_sgl_word_units * 16u; *b_bytes = s->rl_b_sgl_word_units * 16u;
     return BMB200_OK;
 }
 

@@ -265,12 +265,17 @@ int bmb200_set_download(const bmb200_set* set, uint32_t nb_from, uint32_t nb_to,
 /* device addresses of the packed arrays (for torch / NCCL interop) */
 int bmb200_set_device_ptrs(const bmb200_set* set, bmb200_packed_set* out);
 int bmb200_set_free(bmb200_set* set);
-/* bytes of the set's run-list companion (BMB200_TUNE_RUN_LISTS): singles part and long-run part; 0 / 0 while none is built.
- * It is freed with the set. */
+/* size of the set's run-list companion (BMB200_TUNE_RUN_LISTS) in the list form of its entries: 2 bytes per single-bit run and 4
+ * per longer run, each column part padded to 16 bytes.  Singles part and long-run part of part A, the runs of the GAP blocks;
+ * 0 / 0 while none is built.  The long runs are stored in this form; the singles are stored packed (bmb200_set_packed_singles).
+ * The companion is freed with the set. */
 int bmb200_set_run_lists(const bmb200_set* set, uint64_t* sgl_bytes, uint64_t* lr_bytes);
-/* part B of the companion: the listed runs of the set's sparse bit-blocks (singles and long-run bytes) and how many bit-blocks it
- * lists; 0 / 0 / 0 while none is built.  bmb200_set_run_lists reports part A, the runs of the GAP blocks. */
+/* part B of the companion, in the same list form: the listed runs of the set's sparse bit-blocks (singles and long-run bytes) and
+ * how many bit-blocks it lists; 0 / 0 / 0 while none is built. */
 int bmb200_set_bit_run_lists(const bmb200_set* set, uint64_t* sgl_bytes, uint64_t* lr_bytes, uint64_t* listed_blocks);
+/* bytes of the companion's singles as they are resident and streamed, of part A and of part B: 16-byte word units, each holding
+ * the index of one 32-bit word of a block and up to 23 five-bit bit offsets inside it; 0 / 0 while none is built. */
+int bmb200_set_packed_singles(const bmb200_set* set, uint64_t* a_bytes, uint64_t* b_bytes);
 
 /* synthetic input generator (bench / test support): vector v has iid bit density
  * density[v], counter-based RNG keyed by seed[v]; with optimize != 0 every block is

@@ -1,8 +1,9 @@
 """C3's data through the whole-set AND-SUB kernel with the run-list companion (TUNE_RUN_LISTS 1) and without it (0), alternated,
 CUDA events over 20 calls, for an AND group of bit-block vectors ({1, 2}: parts A and B are used) and one with a GAP vector
 ({1, 601}: the companion is not).  Prints ms per call, the bytes each launch streams (unlisted bit-blocks, the companion parts it
-reads, results) next to bench.py's algorithmic bytes (which count every stored block), part B's size and listed blocks, the
-one-time build, popcount / digest equality, and the card it ran on.
+reads, with the singles as streamed: packed word units, or the list form in builds before them) next to bench.py's algorithmic
+bytes (which count every stored block), part B's size and listed blocks, the one-time build, popcount / digest equality, and the
+card it ran on.
 python scripts/bench_run_lists.py   (from the repository root, on an H100)"""
 import json
 import subprocess
@@ -56,6 +57,9 @@ for g0 in ([0, 1], [0, 600]):
             res.free()
     sgl, lr = dset.run_list_bytes()
     bsgl, blr, listed = dset.bit_run_list_bytes()
+    if hasattr(bm.capi.lib(), "bmb200_set_packed_singles"):     # singles as streamed; older builds stream the list form
+        out["list_form_singles"] = {"a": sgl, "b": bsgl}
+        sgl, bsgl = dset.packed_singles_bytes()
     alg = counts["bit"] * 8192 + gap_words * 2 + res_bytes + n_cols * 12
     if g0 == [0, 1]:          # A + B in place of the GAP segments and the listed bit-blocks
         src = (counts["bit"] - listed) * 8192 + sgl + lr + bsgl + blr
