@@ -46,6 +46,7 @@ SYMBOLS = [
     "bmb200_result_fetch_view_async", "bmb200_result_fetch_wait", "bmb200_exchange_mode",
     "bmb200_result_fetch_column", "bmb200_set_run_lists", "bmb200_set_bit_run_lists",
     "bmb200_rank_decompress", "bmb200_rank_compress", "bmb200_scan_str", "bmb200_set_packed_singles",
+    "bmb200_set_run_list_unions",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
@@ -438,6 +439,13 @@ class DeviceSet:
         none is built."""
         a, b = C.c_uint64(0), C.c_uint64(0)
         self.ctx.check(lib().bmb200_set_packed_singles(self._h, C.byref(a), C.byref(b)), "set_packed_singles")
+        return a.value, b.value
+
+    def run_list_unions(self) -> tuple[int, int]:
+        """How many columns stream the companion's part A, and parts A + B, as one 8 KB union mask (those whose part takes 8192
+        streamed bytes or more); (0, 0) while none is built."""
+        a, b = C.c_uint64(0), C.c_uint64(0)
+        self.ctx.check(lib().bmb200_set_run_list_unions(self._h, C.byref(a), C.byref(b)), "set_run_list_unions")
         return a.value, b.value
 
     def stored_bytes(self) -> int:

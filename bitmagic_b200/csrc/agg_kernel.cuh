@@ -1028,7 +1028,8 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
 // its GAP stages unread and applies its GAP blocks straight from global memory.  With the run-list companion (RunLists, passed only
 // when the AND group holds no GAP block) the producer streams the column's companion singles and long runs in place of its GAP segment:
 // part A (the GAP blocks' runs), or A + B (also the runs of the listed bit-blocks, which it then does not stream) when the AND group
-// holds no listed bit-block either.
+// holds no listed bit-block either.  A column whose streamed part has a union mask (RunLists::un_slot) streams that 8 KB mask
+// instead, as one more bit stage that the consumers fold as a SUB-group bit-block: no companion stages, no sweep.
 // Protocol (no wait can outlive the producer): the producer claims a column only when a queue slot is free, publishes (item, #bit
 // stages, GAP bytes, first stage) and then issues all of the column's stages in order, each after its empty barrier; after the last
 // column it publishes an end marker.  Consumers read every queue entry and wait for exactly the stages it announces: every warp
@@ -1078,6 +1079,8 @@ struct RunLists {
     const uint4* sgl;           // singles: word units (runlist_kernel.cuh)
     const uint32_t* lr;         // long runs: FLAT pairs
     const uint32_t* listed;     // bit i: bit-block i of bit_pool is in part B and not streamed; null = stream part A only
+    const uint32_t* un_slot;    // [n_blocks][2]: un_pool slot of the column's U_A / U_AB, ~0 = stream that part packed
+    const uint32_t* un_pool;    // [slots][2048]: the union of the part's runs, streamed as one SUB-group bit stage
 };
 constexpr uint32_t kPipeLstWords = kPipeMaxVec / 32u;       // listed flags of one column's bit-blocks
 
@@ -1094,6 +1097,7 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
     __shared__ __align__(8) uint64_t s_full[kPipeStages], s_empty[kPipeStages], s_qfull[kPipeQueue], s_qempty[kPipeQueue];
     __shared__ uint4 s_q[kPipeQueue];                       // (item | ~0 = end, bit stages, GAP or companion singles bytes, first stage)
     __shared__ uint32_t s_qlr[kPipeQueue];                  // companion long-run bytes (0 without the companion)
+    __shared__ uint32_t s_qun[kPipeQueue];                  // 1: the column's last bit stage is its companion part as a union mask
     __shared__ uint32_t s_lst[kPipeQueue][kPipeLstWords];   // with part B: bit j = the column's bit-block j is listed
     __shared__ uint32_t s_lrk[kPipeQueue][kPipeLstWords];   // ... listed bit-blocks in words < w
     __shared__ uint32_t s_g1[kPipeMaxVec / 32];             // vector -> member of group1 (AND-SUB)
@@ -1128,7 +1132,7 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
             const uint64_t b0 = p.set.bit_base[nb];
             const uint32_t nbit = (uint32_t)(p.set.bit_base[nb + 1] - b0);
             // behind the bit-blocks: the GAP segment (gsrc, gbytes), or the companion's singles (gsrc, gbytes) and long runs (lsrc, lbytes)
-            uint32_t gbytes, lbytes = 0, nlst = 0;
+            uint32_t gbytes, lbytes = 0, nlst = 0, un = 0;
             const uint8_t *gsrc, *lsrc = nullptr;
             if (rl.sgl_base) {
                 const uint64_t s0 = rl.sgl_base[nb], l0 = rl.lr_base[nb];
@@ -1147,13 +1151,21 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
                         s_lst[qs][w] = f; s_lrk[qs][w] = nlst; nlst += __popc(f); r = r1;
                     }
                 }
+                // a union mask stands for the part: one 8 KB stage behind the streamed bit-blocks, which the consumers fold as a
+                // SUB-group bit-block (its role bit is table entry nstr: a union column holds a GAP or listed block, so nstr < M)
+                const uint32_t us = rl.un_slot[2u * nb + (rl.listed ? 1u : 0u)];
+                if (us != ~0u) {
+                    un = 1u; lbytes = 0u; gbytes = kPipeStage;
+                    gsrc = reinterpret_cast<const uint8_t*>(rl.un_pool + (size_t)us * kBlockWords);
+                }
             } else {
                 const uint64_t g0 = p.set.gap_base[nb];
                 gbytes = (uint32_t)((p.set.gap_base[nb + 1] - g0) * 16u);
                 gsrc = reinterpret_cast<const uint8_t*>(p.set.gap_pool + g0 * kGapUnit);
             }
             const uint32_t nstr = nbit - nlst;                   // streamed bit-blocks
-            s_q[qs] = make_uint4(item, nstr, gbytes, seq); s_qlr[qs] = lbytes;
+            if (un && nstr >= kPipeMaxVec) __trap();             // cannot happen (above); the role table would overflow
+            s_q[qs] = make_uint4(item, nstr + un, un ? 0u : gbytes, seq); s_qlr[qs] = lbytes; s_qun[qs] = un;
             mbar_arrive(&s_qfull[qs]);
             const uint8_t* bsrc = reinterpret_cast<const uint8_t*>(p.set.bit_pool + b0 * kBlockWords);
             const uint32_t ng = nstr + (gbytes + kPipeStage - 1u) / kPipeStage, ns = ng + (lbytes + kPipeStage - 1u) / kPipeStage;
@@ -1187,6 +1199,7 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
         const uint32_t lbytes = s_qlr[qs];
         if (e.x == ~0u) break;
         const uint32_t item = e.x, nbit = e.y, gbytes = e.z, seq0 = e.w;
+        if (tid == 0 && s_qun[qs]) atomicOr(&s_brole[b][(nbit - 1u) >> 5], 1u << ((nbit - 1u) & 31u));   // the union stage: SUB
         const uint32_t nb = p.nb_from + item;
         const uint32_t* drow = p.set.desc + (size_t)nb * M;
         const uint16_t* gseg = p.set.gap_pool + p.set.gap_base[nb] * (size_t)kGapUnit;

@@ -124,6 +124,9 @@ struct bmb200_set {
     uint64_t rl_b_sgl_units = 0, rl_b_lr_units = 0, rl_listed_blocks = 0;   // part B
     uint64_t rl_sgl_word_units = 0, rl_b_sgl_word_units = 0;               // the singles as stored: word units of A, of B
     std::vector<uint32_t> listed_vecs;      // bit v: vector v holds a listed bit-block in some column (set with the companion)
+    uint32_t* rl_un_slot = nullptr;         // [n_blocks][2]: union-mask slot of U_A / U_AB (runlist_kernel.cuh), ~0 = none
+    uint32_t* rl_un_pool = nullptr;         // [slots][2048]
+    uint64_t rl_un_a = 0, rl_un_ab = 0;     // columns that stream U_A / U_AB (bmb200_set_run_list_unions)
     size_t cap_desc = 0, cap_base = 0, cap_bit = 0, cap_gap = 0;   // capacities when the arrays came from set_alloc (elements / blocks / units); 0 = not recyclable
 };
 
@@ -223,7 +226,8 @@ void free_set_arrays(bmb200_set* s)
 void free_run_lists(bmb200_set* s)
 {
     cudaFree(s->rl_sgl_base); cudaFree(s->rl_lr_base); cudaFree(s->rl_sgl_mid); cudaFree(s->rl_lr_mid);
-    cudaFree(s->rl_sgl); cudaFree(s->rl_lr); cudaFree(s->rl_listed);
+    cudaFree(s->rl_sgl); cudaFree(s->rl_lr); cudaFree(s->rl_listed); cudaFree(s->rl_un_slot); cudaFree(s->rl_un_pool);
+    s->rl_un_slot = s->rl_un_pool = nullptr; s->rl_un_a = s->rl_un_ab = 0;
     s->rl_sgl_base = s->rl_lr_base = s->rl_sgl_mid = s->rl_lr_mid = nullptr; s->rl_sgl = nullptr; s->rl_lr = nullptr; s->rl_listed = nullptr;
     s->rl_sgl_units = s->rl_lr_units = s->rl_b_sgl_units = s->rl_b_lr_units = s->rl_listed_blocks = 0;
     s->rl_sgl_word_units = s->rl_b_sgl_word_units = 0;
@@ -1337,7 +1341,8 @@ static const std::vector<uint32_t>& gap_vectors(bmb200_ctx* ctx, const bmb200_se
 }
 
 // Builds the run-list companion (runlist_kernel.cuh): count pass (which also lists the sparse bit-blocks), scans, one wait to size
-// the pools, write pass into the zeroed singles pool, then which vectors hold a listed block.  On any failure, or when parts A + B would leave less than
+// the pools, write pass into the zeroed singles pool, then which vectors hold a listed block, then the union masks of the columns
+// whose parts stream a full stage or more.  On any failure, or when parts A + B or the union masks would leave less than
 // kRunListMargin of device memory free, the set is marked as having none (rl_state = -1).
 constexpr size_t kRunListMargin = size_t(1) << 30;
 static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
@@ -1378,8 +1383,34 @@ static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
         ok = cudaGetLastError() == cudaSuccess && cudaMemcpyAsync(h_lv.data(), lv, vwords * 4u, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
              cudaStreamSynchronize(st) == cudaSuccess;
     }
+    // union masks (rl_union_kernel): a slot for each column part that streams at least one full stage, so no column streams more
+    uint64_t n_un_a = 0, n_un_ab = 0;
+    if (ok) {
+        std::vector<uint64_t> sb((size_t)nb + 1), lb((size_t)nb + 1), sm(nb), lm(nb);
+        ok = cudaMemcpyAsync(sb.data(), s->rl_sgl_base, sb.size() * 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaMemcpyAsync(lb.data(), s->rl_lr_base, lb.size() * 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaMemcpyAsync(sm.data(), s->rl_sgl_mid, sm.size() * 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaMemcpyAsync(lm.data(), s->rl_lr_mid, lm.size() * 8, cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaStreamSynchronize(st) == cudaSuccess;
+        std::vector<uint32_t> slot(2 * (size_t)nb, ~0u);
+        uint32_t n_slots = 0;
+        for (uint32_t c = 0; ok && c < nb; ++c) {
+            const uint64_t a = 16u * ((sm[c] - sb[c]) + (lm[c] - lb[c])), ab = 16u * ((sb[c + 1] - sb[c]) + (lb[c + 1] - lb[c]));
+            if (a >= kPipeStage) { slot[2 * c] = n_slots++; ++n_un_a; }
+            if (ab >= kPipeStage) { slot[2 * c + 1] = ab == a ? slot[2 * c] : n_slots++; ++n_un_ab; }
+        }
+        ok = ok && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b >= (size_t)n_slots * kPipeStage + kRunListMargin &&
+             cudaMalloc((void**)&s->rl_un_slot, slot.size() * 4u) == cudaSuccess &&
+             cudaMalloc((void**)&s->rl_un_pool, std::max<size_t>(n_slots, 1u) * kPipeStage) == cudaSuccess &&
+             cudaMemcpyAsync(s->rl_un_slot, slot.data(), slot.size() * 4u, cudaMemcpyHostToDevice, st) == cudaSuccess;
+        if (ok && n_slots)
+            rl_union_kernel<<<nb, kRlThreads, 0, st>>>(s->rl_sgl_base, s->rl_sgl_mid, s->rl_lr_base, s->rl_lr_mid,
+                                                       reinterpret_cast<const uint4*>(s->rl_sgl), s->rl_lr, s->rl_un_slot, s->rl_un_pool);
+        ok = ok && cudaGetLastError() == cudaSuccess && cudaStreamSynchronize(st) == cudaSuccess;
+    }
     cudaFree(wlr); cudaFree(su); cudaFree(lu); cudaFree(tot); cudaFree(lv);
     if (!ok) { cudaGetLastError(); free_run_lists(s); s->rl_state = -1; return false; }
+    s->rl_un_a = n_un_a; s->rl_un_ab = n_un_ab;
     s->rl_sgl_units = h_tot[0]; s->rl_lr_units = h_tot[1];
     s->rl_b_sgl_units = h_tot[2]; s->rl_b_lr_units = h_tot[3]; s->rl_listed_blocks = h_tot[4];
     s->rl_sgl_word_units = h_tot[5]; s->rl_b_sgl_word_units = h_tot[6];
@@ -1402,8 +1433,16 @@ static bool use_run_lists(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_b
     bool part_b = s->rl_listed_blocks != 0;
     for (uint32_t k = a->offsets[0]; part_b && k < a->offsets[1]; ++k)
         if ((s->listed_vecs[a->members[k] >> 5] >> (a->members[k] & 31u)) & 1u) part_b = false;
-    *rl = RunLists{s->rl_sgl_base, s->rl_lr_base, s->rl_sgl_mid, s->rl_lr_mid, reinterpret_cast<const uint4*>(s->rl_sgl), s->rl_lr, part_b ? s->rl_listed : nullptr};
+    *rl = RunLists{s->rl_sgl_base, s->rl_lr_base, s->rl_sgl_mid, s->rl_lr_mid, reinterpret_cast<const uint4*>(s->rl_sgl), s->rl_lr,
+                   part_b ? s->rl_listed : nullptr, s->rl_un_slot, s->rl_un_pool};
     return true;
+}
+
+int bmb200_set_run_list_unions(const bmb200_set* s, uint64_t* a_cols, uint64_t* ab_cols)
+{
+    if (!s || !a_cols || !ab_cols) return BMB200_ERR_BADARG;
+    *a_cols = s->rl_un_a; *ab_cols = s->rl_un_ab;
+    return BMB200_OK;
 }
 
 int bmb200_set_run_lists(const bmb200_set* s, uint64_t* sgl_bytes, uint64_t* lr_bytes)

@@ -19,6 +19,9 @@
 // A + B and skips the listed 8 KB blocks.  Per column, A's and B's units are adjacent in sgl_pool ([sgl_base, sgl_mid) then
 // [sgl_mid, sgl_base[nb+1])), and so are their long runs in lr_pool; each part is packed on its own.  listed: bit i = bit-block i
 // of bit_pool is in part B.
+// Union masks: a column whose part streams at least one full stage (kPipeStage = 8192 bytes of word units and long runs) also
+// keeps that part as one 8 KB bitmap, the union of the runs its sweep clears -- U_A for part A, U_AB for A + B -- and the kernel
+// streams the bitmap in their place (rl_union_kernel below).
 // Order of a part's units: agg_pipe_kernel's sweep gives 16-byte unit u of a column's streamed range (from sgl_base[nb]) to lane
 // u % 32 and issues one atomic per unit on its word, and a warp request is conflict-free when its 32 lanes touch 32 different
 // shared-memory banks of L; word w lies in bank w & 31.  So each part is dealt out by bank: for rounds = min over banks of the
@@ -291,6 +294,51 @@ __global__ void __launch_bounds__(kRlThreads) rl_write_kernel(const SetView v, c
     if (threadIdx.x == 0) { sgl_mid[nb] = sgl_base[nb] + ua; lr_mid[nb] = lr_base[nb] + lcap / 4u; }
     for (uint32_t i = tl + threadIdx.x; i < lcap; i += kRlThreads) lout[i] = 0u;
     for (uint32_t i = tbl + threadIdx.x; i < blcap; i += kRlThreads) blout[i] = 0u;
+}
+
+// Union masks, one CTA per column: un_slot[2 nb] / [2 nb + 1] = the un_pool slot of the column's U_A / U_AB (~0 = none; a column
+// whose part B is empty may name one slot twice).  U_A is every bit the sweep of part A clears, U_AB every bit the sweep of A + B
+// clears: both are decoded from the pools in the sweep's own layout (sgl_unit and flat_quad in agg_kernel.cuh), so a union stage
+// clears exactly what the column's packed stages would.
+__device__ __forceinline__ void rl_union_part(uint32_t* U, const uint4* __restrict__ sgl, uint64_t s0, uint64_t s1,
+                                              const uint32_t* __restrict__ lr, uint64_t l0, uint64_t l1)
+{
+    for (uint64_t i = s0 + threadIdx.x; i < s1; i += kRlThreads) {       // word unit: 23 five-bit offsets inside one word
+        const uint4 q = sgl[i];
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+        uint32_t m = 0;
+#pragma unroll
+        for (int f = 0; f < (int)kSglFields; ++f) m |= 1u << ((w[f / 6] >> (5 * (f % 6))) & 31u);
+        atomicOr(&U[(q.x >> 30) | ((q.y >> 30) << 2) | ((q.z >> 30) << 4) | ((q.w >> 25) << 6)], m);
+    }
+    for (uint64_t i = 4u * l0 + threadIdx.x; i < 4u * l1; i += kRlThreads) {   // FLAT pair (s - 1 | e << 16): bits [s, e]; (0, 0) = none
+        const uint32_t lo = lr[i] & 0xffffu, e = lr[i] >> 16;
+        if (e <= lo) continue;
+        for (uint32_t s = lo + 1u; s <= e; s = (s | 31u) + 1u) {
+            const uint32_t n = min(e - s + 1u, 32u - (s & 31u));
+            atomicOr(&U[s >> 5], (n == 32u ? ~0u : (1u << n) - 1u) << (s & 31u));
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kRlThreads) rl_union_kernel(const uint64_t* __restrict__ sgl_base, const uint64_t* __restrict__ sgl_mid,
+                                                              const uint64_t* __restrict__ lr_base, const uint64_t* __restrict__ lr_mid,
+                                                              const uint4* __restrict__ sgl, const uint32_t* __restrict__ lr,
+                                                              const uint32_t* __restrict__ un_slot, uint32_t* __restrict__ un_pool)
+{
+    __shared__ uint32_t U[kBlockWords];
+    const uint32_t nb = blockIdx.x, sa = un_slot[2u * nb], sab = un_slot[2u * nb + 1u];
+    if (sab == ~0u) return;                                   // U_A implies U_AB: A + B streams no less than A
+    for (uint32_t i = threadIdx.x; i < kBlockWords; i += kRlThreads) U[i] = 0u;
+    __syncthreads();
+    rl_union_part(U, sgl, sgl_base[nb], sgl_mid[nb], lr, lr_base[nb], lr_mid[nb]);
+    __syncthreads();
+    if (sa != ~0u)
+        for (uint32_t i = threadIdx.x; i < kBlockWords; i += kRlThreads) un_pool[(size_t)sa * kBlockWords + i] = U[i];
+    __syncthreads();
+    rl_union_part(U, sgl, sgl_mid[nb], sgl_base[nb + 1], lr, lr_mid[nb], lr_base[nb + 1]);
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < kBlockWords; i += kRlThreads) un_pool[(size_t)sab * kBlockWords + i] = U[i];
 }
 
 // bits[v >> 5] bit (v & 31) = vector v holds a GAP block in some column (bits zeroed before the launch); grid (vector tiles, column slices)

@@ -276,6 +276,9 @@ int bmb200_set_bit_run_lists(const bmb200_set* set, uint64_t* sgl_bytes, uint64_
 /* bytes of the companion's singles as they are resident and streamed, of part A and of part B: 16-byte word units, each holding
  * the index of one 32-bit word of a block and up to 23 five-bit bit offsets inside it; 0 / 0 while none is built. */
 int bmb200_set_packed_singles(const bmb200_set* set, uint64_t* a_bytes, uint64_t* b_bytes);
+/* how many columns stream part A, and parts A + B, of the companion as one 8 KB union mask (the bits the part's runs cover) in
+ * place of the packed part: those whose part takes 8192 bytes or more as streamed; 0 / 0 while none is built. */
+int bmb200_set_run_list_unions(const bmb200_set* set, uint64_t* a_cols, uint64_t* ab_cols);
 
 /* synthetic input generator (bench / test support): vector v has iid bit density
  * density[v], counter-based RNG keyed by seed[v]; with optimize != 0 every block is

@@ -2,8 +2,8 @@
 CUDA events over 20 calls, for an AND group of bit-block vectors ({1, 2}: parts A and B are used) and one with a GAP vector
 ({1, 601}: the companion is not).  Prints ms per call, the bytes each launch streams (unlisted bit-blocks, the companion parts it
 reads, with the singles as streamed: packed word units, or the list form in builds before them) next to bench.py's algorithmic
-bytes (which count every stored block), part B's size and listed blocks, the one-time build, popcount / digest equality, and the
-card it ran on.
+bytes (which count every stored block), part B's size and listed blocks, how many columns stream a union mask (8 KB each, in
+place of their parts), the one-time build, popcount / digest equality, and the card it ran on.
 python scripts/bench_run_lists.py   (from the repository root, on an H100)"""
 import json
 import subprocess
@@ -61,8 +61,13 @@ for g0 in ([0, 1], [0, 600]):
         out["list_form_singles"] = {"a": sgl, "b": bsgl}
         sgl, bsgl = dset.packed_singles_bytes()
     alg = counts["bit"] * 8192 + gap_words * 2 + res_bytes + n_cols * 12
+    un_a, un_ab = dset.run_list_unions() if hasattr(bm.capi.lib(), "bmb200_set_run_list_unions") else (0, 0)
+    out["union_columns"] = {"a": un_a, "ab": un_ab}
     if g0 == [0, 1]:          # A + B in place of the GAP segments and the listed bit-blocks
-        src = (counts["bit"] - listed) * 8192 + sgl + lr + bsgl + blr
+        # a union column streams one 8 KB mask in place of its parts; the parts' sizes are only known summed over the set
+        if un_ab not in (0, n_cols):
+            sys.exit("only some columns stream a union mask: the streamed bytes need per-column part sizes")
+        src = (counts["bit"] - listed) * 8192 + (n_cols * 8192 if un_ab else sgl + lr + bsgl + blr)
     else:
         src = counts["bit"] * 8192 + dset.n_gap_units * 16
     streamed = src + res_bytes + n_cols * 12
