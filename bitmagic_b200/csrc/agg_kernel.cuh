@@ -1030,14 +1030,15 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) agg_kernel(const AggP
 // part A (the GAP blocks' runs), or A + B (also the runs of the listed bit-blocks, which it then does not stream) when the AND group
 // holds no listed bit-block either.  A column whose streamed part has a union mask (RunLists::un_slot) streams that 8 KB mask
 // instead, as one more bit stage that the consumers fold as a SUB-group bit-block: no companion stages, no sweep.
-// Protocol (no wait can outlive the producer): the producer claims a column only when a queue slot is free, publishes (item, #bit
-// stages, GAP bytes, first stage) and then issues all of the column's stages in order, each after its empty barrier; after the last
-// column it publishes an end marker.  Consumers read every queue entry and wait for exactly the stages it announces: every warp
-// waits for every bit stage (two 16-byte words per thread); GAP or companion stage g of the column goes to the kPipeGroup warps of
-// group g % kPipeGroups, each sweeping its kPipeSlice bytes of it.  Every waiter arrives once on the stage's empty barrier, for
-// kPipeWarps / (its waiters) warps, so a stage is free as soon as its slowest slice is done and the rest of the ring stays requested.
-// They free the queue slot once the column is classified, because classification reads the column's listed flags that the
-// producer staged with the entry.  With part B the entry's bit stages are the column's unlisted bit-blocks in order.
+// Protocol (no wait can outlive the producer): the producer warp plans column i + 1 (claim, bases, listed flags) right after it has
+// issued column i's first stage, and publishes (item, #bit stages, GAP bytes, first stage, plan) once a queue slot is free and
+// column i's last stage is issued; after the last column it publishes an end marker.  Consumers read every queue entry, copy it out
+// and free its slot, and wait for exactly the stages it announces: every warp waits for every bit stage (two 16-byte words per
+// thread); GAP or companion stage g of the column goes to the kPipeGroup warps of group g % kPipeGroups, each sweeping its
+// kPipeSlice bytes of it.  Every waiter arrives once on the stage's empty barrier, for kPipeWarps / (its waiters) warps, so a stage
+// is free as soon as its slowest slice is done and the rest of the ring stays requested.  With part B the entry's bit stages are the
+// column's unlisted bit-blocks in order.  With the companion the plan names the AND-group stages (PipeCol) and the consumers skip
+// the descriptor row; a column with no companion stage to sweep (a union column) goes from the bit phase straight to the epilogue.
 // Parity waits are sound because every waiter has waited for every earlier fill of the stage: fills of earlier columns all
 // completed before the column barriers the waiter has passed, and within a column a ring slot is reused only by bit stages,
 // which every warp waits for, or by GAP stages of the same warp group (kPipeStages = 12 is a multiple of kPipeGroups = 4).
@@ -1081,8 +1082,22 @@ struct RunLists {
     const uint32_t* listed;     // bit i: bit-block i of bit_pool is in part B and not streamed; null = stream part A only
     const uint32_t* un_slot;    // [n_blocks][2]: un_pool slot of the column's U_A / U_AB, ~0 = stream that part packed
     const uint32_t* un_pool;    // [slots][2048]: the union of the part's runs, streamed as one SUB-group bit stage
+    const uint16_t* full_cnt;   // [n_blocks]: vectors whose block in column nb is FULL
 };
 constexpr uint32_t kPipeLstWords = kPipeMaxVec / 32u;       // listed flags of one column's bit-blocks
+
+// One column as the producer warp plans it (every lane holds the same values except the AND-member fields).  With the companion
+// the plan also decides what the consumers would otherwise learn from the column's descriptor row: which streamed stages are
+// AND-group bit-blocks (their stream indices, published sorted), how many there are and the result state.
+struct PipeCol {
+    uint32_t item;               // ~0 = no column left
+    uint32_t nstr, nlst, un;     // streamed bit-blocks, listed ones (not streamed), 1 = the companion part is a union mask
+    uint32_t gbytes, lbytes;     // GAP segment or companion singles bytes, companion long-run bytes
+    const uint8_t *bsrc, *gsrc, *lsrc;
+    uint32_t ka, kb;             // stream index of AND member lane / lane + 32 when it is a bit-block, else ~0
+    uint32_t ra, rb;             // ... its position in the sorted index list
+    uint32_t nb0, state;         // AND-group bit-blocks; 0 = NULL, 1 = FULL, 2 = computed (and_state)
+};
 
 __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(const AggParams p, const RunLists rl)
 {
@@ -1097,9 +1112,10 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
     __shared__ __align__(8) uint64_t s_full[kPipeStages], s_empty[kPipeStages], s_qfull[kPipeQueue], s_qempty[kPipeQueue];
     __shared__ uint4 s_q[kPipeQueue];                       // (item | ~0 = end, bit stages, GAP or companion singles bytes, first stage)
     __shared__ uint32_t s_qlr[kPipeQueue];                  // companion long-run bytes (0 without the companion)
-    __shared__ uint32_t s_qun[kPipeQueue];                  // 1: the column's last bit stage is its companion part as a union mask
-    __shared__ uint32_t s_lst[kPipeQueue][kPipeLstWords];   // with part B: bit j = the column's bit-block j is listed
-    __shared__ uint32_t s_lrk[kPipeQueue][kPipeLstWords];   // ... listed bit-blocks in words < w
+    __shared__ uint32_t s_qpl[kPipeQueue];                  // companion plan: AND-group bit-blocks | result state << 16
+    __shared__ uint16_t s_qidx[kPipeQueue][kPipeMaxAndGap]; // ... their stream indices, ascending
+    __shared__ uint32_t s_lst[2][kPipeLstWords];            // producer, with part B: bit j = bit-block j of the column is listed
+    __shared__ uint32_t s_lrk[kPipeLstWords];               // ... listed bit-blocks in words < w of the column being planned
     __shared__ uint32_t s_g1[kPipeMaxVec / 32];             // vector -> member of group1 (AND-SUB)
     __shared__ uint32_t s_brole[2][kPipeMaxVec / 32];       // bit-block j of the column -> group1, one buffer per column parity
     __shared__ uint32_t s_st[2][6];                         // flags, bit0, gap0, AND-group GAP blocks, non-FLAT, first GAP unit
@@ -1117,70 +1133,126 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
     for (uint32_t i = tid; i < kPipeMaxVec / 32; i += kPipeThreads) { s_g1[i] = 0u; s_brole[0][i] = 0u; }
     if (tid < 12) (&s_st[0][0])[tid] = (tid % 6 == 5) ? ~0u : 0u;
     __syncthreads();
-    for (uint32_t k = n0 + tid; k < n0 + n1; k += kPipeThreads) { const uint32_t v = p.group[k]; atomicOr(&s_g1[v >> 5], 1u << (v & 31u)); }
+    if (!rl.sgl_base)                                       // the descriptor-row classification's role table
+        for (uint32_t k = n0 + tid; k < n0 + n1; k += kPipeThreads) { const uint32_t v = p.group[k]; atomicOr(&s_g1[v >> 5], 1u << (v & 31u)); }
     __syncthreads();                                        // the last CTA-wide barrier: the producer warp leaves below
 
-    if (warp == kPipeWarps) {                               // ---- producer (one lane) ----
-        if (lane != 0) return;
-        uint32_t seq = 0;
-        for (uint32_t qi = 0;; ++qi) {
-            const uint32_t qs = qi % kPipeQueue;
-            mbar_wait(&s_qempty[qs], ((qi / kPipeQueue) & 1u) ^ 1u);
-            const uint32_t item = atomicAdd(p.work_counter, 1u);
-            if (item >= p.n_cols) { s_q[qs] = make_uint4(~0u, 0u, 0u, 0u); mbar_arrive(&s_qfull[qs]); return; }
-            const uint32_t nb = p.nb_from + item;
+    if (warp == kPipeWarps) {                               // ---- producer warp ----
+        // AND-group members lane and lane + 32 (the companion plan looks only at them; whole_set() allows at most 64)
+        const uint32_t ma = (uint32_t)lane < n0 ? p.group[lane] : ~0u, mb = (uint32_t)lane + 32u < n0 ? p.group[lane + 32] : ~0u;
+        // Claims the next column and plans it; its listed flags go to s_lst[par].  Three dependent round trips (claim, bases and
+        // AND-member descriptors, listed words), all taken while the previous column's stages are in flight.
+        auto plan = [&](uint32_t par) {
+            PipeCol c{};
+            uint32_t item = 0;
+            if (lane == 0) item = atomicAdd(p.work_counter, 1u);
+            c.item = __shfl_sync(0xffffffffu, item, 0);
+            if (c.item >= p.n_cols) { c.item = ~0u; return c; }
+            const uint32_t nb = p.nb_from + c.item;
             const uint64_t b0 = p.set.bit_base[nb];
             const uint32_t nbit = (uint32_t)(p.set.bit_base[nb + 1] - b0);
+            c.bsrc = reinterpret_cast<const uint8_t*>(p.set.bit_pool + b0 * kBlockWords);
+            c.ka = c.kb = ~0u;
             // behind the bit-blocks: the GAP segment (gsrc, gbytes), or the companion's singles (gsrc, gbytes) and long runs (lsrc, lbytes)
-            uint32_t gbytes, lbytes = 0, nlst = 0, un = 0;
-            const uint8_t *gsrc, *lsrc = nullptr;
             if (rl.sgl_base) {
+                const uint32_t* drow = p.set.desc + (size_t)nb * M;
+                const uint32_t da = ma != ~0u ? drow[ma] : 0u, db = mb != ~0u ? drow[mb] : 0u;
+                const uint32_t nfull = rl.full_cnt[nb];
                 const uint64_t s0 = rl.sgl_base[nb], l0 = rl.lr_base[nb];
                 const uint64_t s1 = rl.listed ? rl.sgl_base[nb + 1] : rl.sgl_mid[nb], l1 = rl.listed ? rl.lr_base[nb + 1] : rl.lr_mid[nb];
-                gbytes = (uint32_t)((s1 - s0) * 16u); lbytes = (uint32_t)((l1 - l0) * 16u);
-                gsrc = reinterpret_cast<const uint8_t*>(rl.sgl + s0); lsrc = reinterpret_cast<const uint8_t*>(rl.lr + l0 * 4u);
-                if (rl.listed) {        // stage the column's listed flags (bit j = bit-block j) and their running counts for everyone
+                const uint32_t us = rl.un_slot[2u * nb + (rl.listed ? 1u : 0u)];
+                c.gbytes = (uint32_t)((s1 - s0) * 16u); c.lbytes = (uint32_t)((l1 - l0) * 16u);
+                c.gsrc = reinterpret_cast<const uint8_t*>(rl.sgl + s0); c.lsrc = reinterpret_cast<const uint8_t*>(rl.lr + l0 * 4u);
+                if (rl.listed) {        // the column's listed flags (bit j = bit-block j) and their running counts, 32 words per step
                     const uint32_t* lw = rl.listed + (b0 >> 5);
                     const uint32_t sh = (uint32_t)b0 & 31u, nw = (nbit + 31u) / 32u;
-                    uint32_t r = lw[0];
-#pragma unroll 4
-                    for (uint32_t w = 0; w < nw; ++w) {
-                        const uint32_t r1 = lw[w + 1u];
-                        uint32_t f = __funnelshift_r(r, r1, sh);
+                    for (uint32_t w0 = 0; w0 < nw; w0 += 32u) {
+                        const uint32_t w = w0 + (uint32_t)lane;
+                        uint32_t f = w < nw ? __funnelshift_r(lw[w], lw[w + 1u], sh) : 0u;
                         if (32u * w + 32u > nbit) f &= (1u << (nbit & 31u)) - 1u;
-                        s_lst[qs][w] = f; s_lrk[qs][w] = nlst; nlst += __popc(f); r = r1;
+                        uint32_t x = __popc(f);
+#pragma unroll
+                        for (uint32_t o = 1; o < 32u; o <<= 1) { const uint32_t y = __shfl_up_sync(0xffffffffu, x, o); if ((uint32_t)lane >= o) x += y; }
+                        if (w < nw) { s_lst[par][w] = f; s_lrk[w] = c.nlst + x - __popc(f); }
+                        c.nlst += __shfl_sync(0xffffffffu, x, 31);
                     }
+                    __syncwarp();
                 }
-                // a union mask stands for the part: one 8 KB stage behind the streamed bit-blocks, which the consumers fold as a
-                // SUB-group bit-block (its role bit is table entry nstr: a union column holds a GAP or listed block, so nstr < M)
-                const uint32_t us = rl.un_slot[2u * nb + (rl.listed ? 1u : 0u)];
+                // a union mask stands for the part: one 8 KB stage behind the streamed bit-blocks, folded as a SUB-group bit-block
                 if (us != ~0u) {
-                    un = 1u; lbytes = 0u; gbytes = kPipeStage;
-                    gsrc = reinterpret_cast<const uint8_t*>(rl.un_pool + (size_t)us * kBlockWords);
+                    c.un = 1u; c.lbytes = 0u; c.gbytes = kPipeStage;
+                    c.gsrc = reinterpret_cast<const uint8_t*>(rl.un_pool + (size_t)us * kBlockWords);
+                }
+                // AND members: stream index of a bit-block = rel minus the listed blocks below it (an AND member is never listed:
+                // use_run_lists streams part B only then); NULL and FULL members decide the state; the companion rule leaves no GAP
+                auto key = [&](uint32_t m, uint32_t d) -> uint32_t {
+                    if (m == ~0u || (d & 3u) != BMB200_BLK_BIT) return ~0u;
+                    uint32_t j = (d >> 2) & kRelMask;
+                    if (rl.listed) j -= s_lrk[j >> 5] + __popc(s_lst[par][j >> 5] & ((1u << (j & 31u)) - 1u));
+                    return j;
+                };
+                c.ka = key(ma, da); c.kb = key(mb, db);
+                const uint32_t null0 = __ballot_sync(0xffffffffu, (ma != ~0u && (da & 3u) == BMB200_BLK_NULL) ||
+                                                                  (mb != ~0u && (db & 3u) == BMB200_BLK_NULL));
+                const uint32_t full0 = __popc(__ballot_sync(0xffffffffu, ma != ~0u && (da & 3u) == BMB200_BLK_FULL)) +
+                                       __popc(__ballot_sync(0xffffffffu, mb != ~0u && (db & 3u) == BMB200_BLK_FULL));
+                c.nb0 = __popc(__ballot_sync(0xffffffffu, c.ka != ~0u)) + __popc(__ballot_sync(0xffffffffu, c.kb != ~0u));
+                c.state = (null0 || n0 == 0u || nfull > full0) ? 0u : (c.nb0 == 0u && n1 == 0u) ? 1u : 2u;   // nfull > full0: a SUB block is FULL
+                for (uint32_t k = 0; k < n0; ++k) {               // sorted position: the indices are distinct, ~0 sorts last
+                    const uint32_t x = __shfl_sync(0xffffffffu, k < 32u ? c.ka : c.kb, k & 31u);
+                    c.ra += x < c.ka; c.rb += x < c.kb;
                 }
             } else {
                 const uint64_t g0 = p.set.gap_base[nb];
-                gbytes = (uint32_t)((p.set.gap_base[nb + 1] - g0) * 16u);
-                gsrc = reinterpret_cast<const uint8_t*>(p.set.gap_pool + g0 * kGapUnit);
+                c.gbytes = (uint32_t)((p.set.gap_base[nb + 1] - g0) * 16u);
+                c.gsrc = reinterpret_cast<const uint8_t*>(p.set.gap_pool + g0 * kGapUnit);
             }
-            const uint32_t nstr = nbit - nlst;                   // streamed bit-blocks
-            if (un && nstr >= kPipeMaxVec) __trap();             // cannot happen (above); the role table would overflow
-            s_q[qs] = make_uint4(item, nstr + un, un ? 0u : gbytes, seq); s_qlr[qs] = lbytes; s_qun[qs] = un;
-            mbar_arrive(&s_qfull[qs]);
-            const uint8_t* bsrc = reinterpret_cast<const uint8_t*>(p.set.bit_pool + b0 * kBlockWords);
-            const uint32_t ng = nstr + (gbytes + kPipeStage - 1u) / kPipeStage, ns = ng + (lbytes + kPipeStage - 1u) / kPipeStage;
-            for (uint32_t j = 0, jb = 0; j < ns; ++j, ++seq) {
-                const uint32_t s = seq % kPipeStages;
-                if (j < nstr && nlst)                            // the next unlisted bit-block
-                    while ((s_lst[qs][jb >> 5] >> (jb & 31u)) & 1u) ++jb;
-                mbar_wait(&s_empty[s], ((seq / kPipeStages) & 1u) ^ 1u);
-                uint32_t bytes; const uint8_t* src;
-                if (j < nstr)    { bytes = kPipeStage; src = bsrc + (size_t)jb++ * kPipeStage; }
-                else if (j < ng) { const uint32_t o = (j - nstr) * kPipeStage; bytes = min(kPipeStage, gbytes - o); src = gsrc + o; }
-                else             { const uint32_t o = (j - ng) * kPipeStage;   bytes = min(kPipeStage, lbytes - o); src = lsrc + o; }
-                mbar_arrive_expect_tx(&s_full[s], bytes);
-                bulk_g2s(ring + (size_t)s * kPipeStage, src, bytes, &s_full[s]);
+            c.nstr = nbit - c.nlst;
+            return c;
+        };
+        // With the companion, column i's plan is made right after column i - 1's first stage is issued and published after its
+        // last: no global round trip separates the two columns' stages.  The GAP-segment path plans after the last stage, as its
+        // columns are long enough to hide the round trips and a column claimed a whole column early unbalances the tail.  The
+        // first trip streams nothing and plans column 0.
+        PipeCol cur{};
+        uint32_t seq = 0;
+        for (uint32_t qi = 0;; ++qi) {
+            const uint32_t par = qi & 1u, ng = cur.nstr + (cur.gbytes + kPipeStage - 1u) / kPipeStage;
+            const uint32_t ns = ng + (cur.lbytes + kPipeStage - 1u) / kPipeStage, jp = rl.sgl_base ? 0u : max(ns, 1u) - 1u;
+            PipeCol nxt;
+            for (uint32_t j = 0, jb = 0; j < max(ns, 1u); ++j) {
+                if (j < ns) {
+                    const uint32_t s = seq % kPipeStages;
+                    if (j < cur.nstr && cur.nlst)                // the next unlisted bit-block
+                        while ((s_lst[par ^ 1u][jb >> 5] >> (jb & 31u)) & 1u) ++jb;
+                    mbar_wait(&s_empty[s], ((seq / kPipeStages) & 1u) ^ 1u);
+                    uint32_t bytes; const uint8_t* src;
+                    if (j < cur.nstr) { bytes = kPipeStage; src = cur.bsrc + (size_t)jb++ * kPipeStage; }
+                    else if (j < ng)  { const uint32_t o = (j - cur.nstr) * kPipeStage; bytes = min(kPipeStage, cur.gbytes - o); src = cur.gsrc + o; }
+                    else              { const uint32_t o = (j - ng) * kPipeStage;       bytes = min(kPipeStage, cur.lbytes - o); src = cur.lsrc + o; }
+                    if (lane == 0) {
+                        mbar_arrive_expect_tx(&s_full[s], bytes);
+                        bulk_g2s(ring + (size_t)s * kPipeStage, src, bytes, &s_full[s]);
+                    }
+                    ++seq;
+                }
+                if (j == jp) nxt = plan(par);
             }
+            const uint32_t qs = qi % kPipeQueue;
+            mbar_wait(&s_qempty[qs], ((qi / kPipeQueue) & 1u) ^ 1u);
+            if (nxt.item == ~0u) {
+                if (lane == 0) { s_q[qs] = make_uint4(~0u, 0u, 0u, 0u); mbar_arrive(&s_qfull[qs]); }
+                return;
+            }
+            if (nxt.ka != ~0u) s_qidx[qs][nxt.ra] = (uint16_t)nxt.ka;
+            if (nxt.kb != ~0u) s_qidx[qs][nxt.rb] = (uint16_t)nxt.kb;
+            if (lane == 0) {
+                s_q[qs] = make_uint4(nxt.item, nxt.nstr + nxt.un, nxt.un ? 0u : nxt.gbytes, seq);
+                s_qlr[qs] = nxt.lbytes; s_qpl[qs] = nxt.nb0 | (nxt.state << 16);
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&s_qfull[qs]);
+            cur = nxt;
         }
     }
 
@@ -1190,24 +1262,35 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
     asm volatile("mov.u32 %0, %1;" : "=r"(Ks) : "r"(smem_u32(K)));
     asm volatile("mov.u32 %0, %1;" : "=r"(ring_s) : "r"(smem_u32(ring)));
     constexpr int H = kPipeWpt / 4;
+    const bool planned = rl.sgl_base != nullptr;             // the companion path: the producer's plan replaces the classification
     for (uint32_t qi = 0;; ++qi) {
         const uint32_t b = qi & 1u, qs = qi % kPipeQueue;
-        if (tid < 6) s_st[b ^ 1u][tid] = (tid == 5) ? ~0u : 0u;          // next column's counters (nobody reads them any more)
-        if (tid < (int)(kPipeMaxVec / 32)) s_brole[b ^ 1u][tid] = 0u;
+        if (!planned) {
+            if (tid < 6) s_st[b ^ 1u][tid] = (tid == 5) ? ~0u : 0u;      // next column's counters (nobody reads them any more)
+            if (tid < (int)(kPipeMaxVec / 32)) s_brole[b ^ 1u][tid] = 0u;
+        }
         mbar_wait(&s_qfull[qs], (qi / kPipeQueue) & 1u);
         const uint4 e = s_q[qs];
-        const uint32_t lbytes = s_qlr[qs];
         if (e.x == ~0u) break;
         const uint32_t item = e.x, nbit = e.y, gbytes = e.z, seq0 = e.w;
-        if (tid == 0 && s_qun[qs]) atomicOr(&s_brole[b][(nbit - 1u) >> 5], 1u << ((nbit - 1u) & 31u));   // the union stage: SUB
+        const uint32_t lbytes = s_qlr[qs], pl = s_qpl[qs], pnb0 = pl & 0xffffu;
+        // the plan's AND stream indices, entries lane and lane + 32 (copied out, so the slot is free for the producer right away)
+        const uint32_t ia = (uint32_t)lane < pnb0 ? s_qidx[qs][lane] : ~0u, ib = (uint32_t)lane + 32u < pnb0 ? s_qidx[qs][lane + 32] : ~0u;
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&s_qempty[qs]);
         const uint32_t nb = p.nb_from + item;
         const uint32_t* drow = p.set.desc + (size_t)nb * M;
         const uint16_t* gseg = p.set.gap_pool + p.set.gap_base[nb] * (size_t)kGapUnit;
+        int state = (int)(pl >> 16);
+        uint32_t nag = 0;
+        bool flat = false;
+        uint32_t lead = 0;
 
         // ---- classification by vector (every vector is a member: no member list to resolve); vector tid + 256 i is trip i ----
         // The descriptors are dropped after it: the rare paths behind the bit phase re-read the row.  `lead` keeps the one fact
         // the FLAT path needs from it, bit i = trip i's vector is a SUB-group GAP block without lead pad.
-        uint32_t fl = 0, nb0 = 0, ng0 = 0, nonflat = 0, lo = ~0u, lead = 0;
+        if (!planned) {
+        uint32_t fl = 0, nb0 = 0, ng0 = 0, nonflat = 0, lo = ~0u;
         {
             uint32_t dv[kPipePerThr];
 #pragma unroll
@@ -1222,14 +1305,8 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
                 const uint32_t d = dv[i], kind = d & 3u;
                 const bool g1 = (s_g1[v >> 5] >> (v & 31u)) & 1u;
                 if (kind == BMB200_BLK_BIT) {
-                    // role by streamed index: rel minus the listed blocks below it (a listed block is a SUB-group block, never streamed)
-                    if (g1) {
-                        uint32_t j = (d >> 2) & (kPipeMaxVec - 1u);
-                        if (rl.listed) {
-                            const uint32_t f = s_lst[qs][j >> 5], below = f & ((1u << (j & 31u)) - 1u);
-                            if ((f >> (j & 31u)) & 1u) continue;
-                            j -= s_lrk[qs][j >> 5] + __popc(below);
-                        }
+                    if (g1) {                                             // without the companion, stage j is bit-block j
+                        const uint32_t j = (d >> 2) & (kPipeMaxVec - 1u);
                         atomicOr(&s_brole[b][j >> 5], 1u << (j & 31u));
                     } else {
                         ++nb0;
@@ -1263,26 +1340,46 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
             if (lo != ~0u) atomicMin(&s_st[b][5], lo);
         }
         agg_sync<true, kPipeConsumers>();
-        if (lane == 0) mbar_arrive(&s_qempty[qs]);               // the entry and its listed flags are read: the slot may be refilled
         // FLAT: the whole GAP segment is a flat window of 1-run sources (headers, pads and tail fill decode to empty runs)
-        const bool flat = s_st[b][4] == 0u && s_st[b][5] == 0u;
-        const uint32_t nag = s_st[b][3];                         // <= kPipeMaxAndGap when flat
+        flat = s_st[b][4] == 0u && s_st[b][5] == 0u;
+        nag = s_st[b][3];                                        // <= kPipeMaxAndGap when flat
+        state = and_state<OP>(s_st[b][0], s_st[b][1], s_st[b][2], n0, n1);
+        }
 
         // ---- bit phase: stage j = bit-block j of the column, two LDS.128 per thread ----
+        // Planned: stage j is an AND-group bit-block when it is the plan's next index (ascending); every other stage is SUB.
         uint4 acc0[H], acc1[H];
 #pragma unroll
         for (int h = 0; h < H; ++h) { acc0[h] = make_uint4(~0u, ~0u, ~0u, ~0u); acc1[h] = make_uint4(0u, 0u, 0u, 0u); }
+        uint32_t na = 0, and_j = __shfl_sync(0xffffffffu, ia, 0);
         for (uint32_t j = 0; j < nbit; ++j) {
             const uint32_t sq = seq0 + j, s = sq % kPipeStages;
             mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
             uint4 v[H];
 #pragma unroll
             for (int h = 0; h < H; ++h) v[h] = lds128(ring_s + s * kPipeStage + (uint32_t)(h * kPipeConsumers + tid) * 16u);
-            const bool sub = (s_brole[b][j >> 5] >> (j & 31u)) & 1u;
+            bool sub;
+            if (planned) {
+                sub = j != and_j;
+                if (!sub) { ++na; and_j = __shfl_sync(0xffffffffu, na < 32u ? ia : ib, na & 31u); }
+            } else {
+                sub = (s_brole[b][j >> 5] >> (j & 31u)) & 1u;
+            }
 #pragma unroll
             for (int h = 0; h < H; ++h) { if (sub) acc_or(acc1[h], v[h]); else acc_apply0<OP>(acc0[h], v[h]); }
             __syncwarp();
             if (lane == 0) mbar_arrive(&s_empty[s]);
+        }
+        // the GAP phase's stages: the GAP segment, or the companion's singles and long-run stages (none on a union column)
+        const uint32_t ngs = (gbytes + kPipeStage - 1u) / kPipeStage, nst = ngs + (lbytes + kPipeStage - 1u) / kPipeStage;
+        Quads<H> R;
+        if (planned && nst == 0u) {      // nothing to sweep: the folded registers are the result, no live mask and no GAP-phase barriers
+#pragma unroll
+            for (int h = 0; h < H; ++h)
+                R.q[h] = state == 0 ? make_uint4(0u, 0u, 0u, 0u) : state == 1 ? make_uint4(~0u, ~0u, ~0u, ~0u)
+                       : make_uint4(acc0[h].x & ~acc1[h].x, acc0[h].y & ~acc1[h].y, acc0[h].z & ~acc1[h].z, acc0[h].w & ~acc1[h].w);
+            finish_block<true, true, kPipeWpt>(p, item, item, 0u, R, state, K, s_pc, s_tr, s_dg);
+            continue;
         }
         // live mask L = AND of the AND-group bit-blocks minus the SUB-group ones (every bit a candidate without bit-blocks)
 #pragma unroll
@@ -1291,12 +1388,10 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
         agg_sync<true, kPipeConsumers>();
 
         // ---- GAP phase: GAP stage g goes to warp group g % kPipeGroups; a warp sweeps bytes [wlo, wlo + kPipeSlice) of it ----
-        const uint32_t ngs = (gbytes + kPipeStage - 1u) / kPipeStage;
         const uint32_t grp = (uint32_t)warp / kPipeGroup, wlo = ((uint32_t)warp % kPipeGroup) * kPipeSlice;
-        if (rl.sgl_base) {
+        if (planned) {
             // run-list companion: every GAP block is a SUB-group block, so the phase clears the column's singles (stages 0 .. ngs-1)
             // and long runs (the stages behind them) from L; no lead-pad repair, no AND-group blocks
-            const uint32_t nst = ngs + (lbytes + kPipeStage - 1u) / kPipeStage;
             uint32_t flat_mode = 0;
             for (uint32_t g = grp; g < nst; g += kPipeGroups) {
                 const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
@@ -1366,8 +1461,6 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
         agg_sync<true, kPipeConsumers>();
 
         // ---- epilogue ----
-        const int state = and_state<OP>(s_st[b][0], s_st[b][1], s_st[b][2], n0, n1);
-        Quads<H> R;
 #pragma unroll
         for (int h = 0; h < H; ++h)
             R.q[h] = state == 0 ? make_uint4(0u, 0u, 0u, 0u) : state == 1 ? make_uint4(~0u, ~0u, ~0u, ~0u) : K4[h * kPipeConsumers + tid];

@@ -126,6 +126,7 @@ struct bmb200_set {
     std::vector<uint32_t> listed_vecs;      // bit v: vector v holds a listed bit-block in some column (set with the companion)
     uint32_t* rl_un_slot = nullptr;         // [n_blocks][2]: union-mask slot of U_A / U_AB (runlist_kernel.cuh), ~0 = none
     uint32_t* rl_un_pool = nullptr;         // [slots][2048]
+    uint16_t* rl_full = nullptr;            // [n_blocks]: FULL blocks per column
     uint64_t rl_un_a = 0, rl_un_ab = 0;     // columns that stream U_A / U_AB (bmb200_set_run_list_unions)
     size_t cap_desc = 0, cap_base = 0, cap_bit = 0, cap_gap = 0;   // capacities when the arrays came from set_alloc (elements / blocks / units); 0 = not recyclable
 };
@@ -227,6 +228,7 @@ void free_run_lists(bmb200_set* s)
 {
     cudaFree(s->rl_sgl_base); cudaFree(s->rl_lr_base); cudaFree(s->rl_sgl_mid); cudaFree(s->rl_lr_mid);
     cudaFree(s->rl_sgl); cudaFree(s->rl_lr); cudaFree(s->rl_listed); cudaFree(s->rl_un_slot); cudaFree(s->rl_un_pool);
+    cudaFree(s->rl_full); s->rl_full = nullptr;
     s->rl_un_slot = s->rl_un_pool = nullptr; s->rl_un_a = s->rl_un_ab = 0;
     s->rl_sgl_base = s->rl_lr_base = s->rl_sgl_mid = s->rl_lr_mid = nullptr; s->rl_sgl = nullptr; s->rl_lr = nullptr; s->rl_listed = nullptr;
     s->rl_sgl_units = s->rl_lr_units = s->rl_b_sgl_units = s->rl_b_lr_units = s->rl_listed_blocks = 0;
@@ -1359,11 +1361,12 @@ static bool build_run_lists(bmb200_ctx* ctx, bmb200_set* s)
               cudaMalloc((void**)&s->rl_sgl_base, ((size_t)nb + 1) * 8) == cudaSuccess &&
               cudaMalloc((void**)&s->rl_lr_base, ((size_t)nb + 1) * 8) == cudaSuccess &&
               cudaMalloc((void**)&s->rl_sgl_mid, (size_t)nb * 8) == cudaSuccess && cudaMalloc((void**)&s->rl_lr_mid, (size_t)nb * 8) == cudaSuccess &&
+              cudaMalloc((void**)&s->rl_full, (size_t)nb * 2) == cudaSuccess &&
               cudaMalloc((void**)&s->rl_listed, lwords * 4u) == cudaSuccess &&
               cudaMemsetAsync(s->rl_listed, 0, lwords * 4u, st) == cudaSuccess && cudaMemsetAsync(tot, 0, sizeof(h_tot), st) == cudaSuccess &&
               cudaMemsetAsync(lv, 0, vwords * 4u, st) == cudaSuccess;
     if (ok) {
-        rl_count_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wlr, su, lu, s->rl_listed, tot);
+        rl_count_kernel<<<nb, kRlThreads, 0, st>>>(s->v, wlr, su, lu, s->rl_listed, s->rl_full, tot);
         scan_u64_kernel<<<1, 1024, 0, st>>>(su, nb, s->rl_sgl_base);
         scan_u64_kernel<<<1, 1024, 0, st>>>(lu, nb, s->rl_lr_base);
         ok = cudaGetLastError() == cudaSuccess && cudaMemcpyAsync(h_tot, tot, sizeof(h_tot), cudaMemcpyDeviceToHost, st) == cudaSuccess &&
@@ -1434,7 +1437,7 @@ static bool use_run_lists(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_b
     for (uint32_t k = a->offsets[0]; part_b && k < a->offsets[1]; ++k)
         if ((s->listed_vecs[a->members[k] >> 5] >> (a->members[k] & 31u)) & 1u) part_b = false;
     *rl = RunLists{s->rl_sgl_base, s->rl_lr_base, s->rl_sgl_mid, s->rl_lr_mid, reinterpret_cast<const uint4*>(s->rl_sgl), s->rl_lr,
-                   part_b ? s->rl_listed : nullptr, s->rl_un_slot, s->rl_un_pool};
+                   part_b ? s->rl_listed : nullptr, s->rl_un_slot, s->rl_un_pool, s->rl_full};
     return true;
 }
 

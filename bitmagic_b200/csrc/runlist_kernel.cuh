@@ -102,8 +102,9 @@ __device__ __forceinline__ void rl_block(const uint16_t* __restrict__ g, uint32_
 }
 
 // Warp w of a column takes vectors [w * per, (w + 1) * per): its long runs land in vector order behind those of warps < w.
+// nfull (unless null) grows by the warp's FULL blocks.
 __device__ __forceinline__ void rl_column(const SetView v, uint32_t nb, uint32_t warp, uint32_t lane, uint32_t& ns, uint32_t& nl,
-                                          const SglOut& so, uint32_t* lout)
+                                          const SglOut& so, uint32_t* lout, uint32_t* nfull = nullptr)
 {
     const uint32_t M = v.n_vec, per = (M + kRlWarps - 1u) / kRlWarps;
     const uint32_t* drow = v.desc + (size_t)nb * M;
@@ -112,6 +113,7 @@ __device__ __forceinline__ void rl_column(const SetView v, uint32_t nb, uint32_t
         const uint32_t x = v0 + lane;
         const uint32_t d = (x < min(M, (warp + 1u) * per)) ? drow[x] : BMB200_BLK_NULL;
         uint32_t m = __ballot_sync(0xffffffffu, (d & 3u) == BMB200_BLK_GAP);
+        if (nfull) *nfull += __popc(__ballot_sync(0xffffffffu, (d & 3u) == BMB200_BLK_FULL));
         while (m) {
             const int l = __ffs(m) - 1; m &= m - 1u;
             const uint32_t dl = __shfl_sync(0xffffffffu, d, l);
@@ -217,34 +219,36 @@ __device__ __forceinline__ void rl_deal(const uint32_t* cnt, uint32_t* ust, uint
     __syncthreads();
 }
 
-// pass 1, one CTA per column: per-warp long-run counts wlr[nb][w] of part A and wlr[nb][kRlWarps + w] of part B, the listed flags
+// pass 1, one CTA per column: per-warp long-run counts wlr[nb][w] of part A and wlr[nb][kRlWarps + w] of part B, the column's
+// FULL blocks full_cnt[nb] (agg_pipe_kernel's plan: a SUB-group block is FULL when the AND group holds fewer), the listed flags
 // (zeroed before the launch), the column's word units (A + B) and long-run units, and the set's totals tot = (A singles units,
 // A long-run units, B singles units, B long-run units in the list form, listed blocks, A word units, B word units), zeroed before
 // the launch.  The list form keeps 8 singles and 4 long runs per 16-byte unit, each column part padded on its own.
 __global__ void __launch_bounds__(kRlThreads) rl_count_kernel(const SetView v, uint32_t* __restrict__ wlr, uint64_t* __restrict__ sgl_units,
                                                               uint64_t* __restrict__ lr_units, uint32_t* __restrict__ listed,
-                                                              unsigned long long* __restrict__ tot)
+                                                              uint16_t* __restrict__ full_cnt, unsigned long long* __restrict__ tot)
 {
-    __shared__ uint32_t s_cnt[2][kBlockWords], s_ust[kBlockWords], s_c[4][kRlWarps], s_n[kRlWarps], s_ub[32], s_lb[32], s_du[2][2];
+    __shared__ uint32_t s_cnt[2][kBlockWords], s_ust[kBlockWords], s_c[5][kRlWarps], s_n[kRlWarps], s_ub[32], s_lb[32], s_du[2][2];
     const uint32_t nb = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
     for (uint32_t i = threadIdx.x; i < 2u * kBlockWords; i += kRlThreads) (&s_cnt[0][0])[i] = 0u;
     __syncthreads();
-    uint32_t ns = 0, nl = 0, bs = 0, bl = 0, nlst = 0;
-    rl_column(v, nb, warp, lane, ns, nl, SglOut{nullptr, s_cnt[0]}, nullptr);
+    uint32_t ns = 0, nl = 0, bs = 0, bl = 0, nlst = 0, nfull = 0;
+    rl_column(v, nb, warp, lane, ns, nl, SglOut{nullptr, s_cnt[0]}, nullptr, &nfull);
     rl_bits<true>(v, nb, warp, lane, bs, bl, nlst, listed, SglOut{nullptr, s_cnt[1]}, nullptr);
     if (lane == 0) {
-        s_c[0][warp] = ns; s_c[1][warp] = nl; s_c[2][warp] = bs; s_c[3][warp] = bl; s_n[warp] = nlst;
+        s_c[0][warp] = ns; s_c[1][warp] = nl; s_c[2][warp] = bs; s_c[3][warp] = bl; s_c[4][warp] = nfull; s_n[warp] = nlst;
         wlr[(size_t)nb * kRlCnt + warp] = nl; wlr[(size_t)nb * kRlCnt + kRlWarps + warp] = bl;
     }
     __syncthreads();
     rl_deal(s_cnt[0], s_ust, s_ub, s_lb, s_du[0], warp, lane);
     rl_deal(s_cnt[1], s_ust, s_ub, s_lb, s_du[1], warp, lane);
     if (threadIdx.x == 0) {
-        uint32_t t[5] = {0, 0, 0, 0, 0};
+        uint32_t t[5] = {0, 0, 0, 0, 0}, f = 0;
         for (int w = 0; w < kRlWarps; ++w) {
             for (int k = 0; k < 4; ++k) t[k] += s_c[k][w];
-            t[4] += s_n[w];
+            t[4] += s_n[w]; f += s_c[4][w];
         }
+        full_cnt[nb] = (uint16_t)f;
         const uint32_t u[7] = {(t[0] + 7u) / 8u, (t[1] + 3u) / 4u, (t[2] + 7u) / 8u, (t[3] + 3u) / 4u, t[4], s_du[0][1], s_du[1][1]};
         sgl_units[nb] = u[5] + u[6];
         lr_units[nb] = u[1] + u[3];
