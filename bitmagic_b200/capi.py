@@ -46,11 +46,11 @@ SYMBOLS = [
     "bmb200_result_fetch_view_async", "bmb200_result_fetch_wait", "bmb200_exchange_mode",
     "bmb200_result_fetch_column", "bmb200_set_run_lists", "bmb200_set_bit_run_lists",
     "bmb200_rank_decompress", "bmb200_rank_compress", "bmb200_scan_str", "bmb200_set_packed_singles",
-    "bmb200_set_run_list_unions",
+    "bmb200_set_run_list_unions", "bmb200_set_coverage",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
-TUNE_GAP_MODE, TUNE_CTAS_PER_SM, TUNE_HOST_THREADS, TUNE_AGG_PIPELINE, TUNE_RUN_LISTS = 0, 1, 2, 3, 4
+TUNE_GAP_MODE, TUNE_CTAS_PER_SM, TUNE_HOST_THREADS, TUNE_AGG_PIPELINE, TUNE_RUN_LISTS, TUNE_COVERAGE = 0, 1, 2, 3, 4, 5
 
 
 class PackedSetC(C.Structure):
@@ -446,6 +446,13 @@ class DeviceSet:
         streamed bytes or more); (0, 0) while none is built."""
         a, b = C.c_uint64(0), C.c_uint64(0)
         self.ctx.check(lib().bmb200_set_run_list_unions(self._h, C.byref(a), C.byref(b)), "set_run_list_unions")
+        return a.value, b.value
+
+    def coverage(self, n0: int) -> tuple[int, int]:
+        """(columns storing an 8 KB plane, columns covered everywhere) of the set's coverage plane for AND groups of n0 members;
+        (0, 0) while none is built (TUNE_COVERAGE)."""
+        a, b = C.c_uint64(0), C.c_uint64(0)
+        self.ctx.check(lib().bmb200_set_coverage(self._h, C.c_uint32(n0), C.byref(a), C.byref(b)), "set_coverage")
         return a.value, b.value
 
     def stored_bytes(self) -> int:

@@ -36,6 +36,7 @@
 //   * epilogue fuses popcount, 64-wave digest, run count and the result-kind decision.
 #pragma once
 #include "common.cuh"
+#include "coverage_kernel.cuh"
 #include <type_traits>
 
 namespace bmb200 {
@@ -1086,6 +1087,14 @@ struct RunLists {
 };
 constexpr uint32_t kPipeLstWords = kPipeMaxVec / 32u;       // listed flags of one column's bit-blocks
 
+// The coverage plane GT_n0 of the set for this call's AND-group size (coverage_kernel.cuh), or all null.  The host passes it only
+// when no GAP block of the set belongs to the AND group; the kernel then streams each column's AND-group bit-blocks and the
+// column's plane slot (unless kCovZero), folded as a SUB-group bit-block, and nothing else.
+struct Coverage {
+    const uint32_t* slot;       // [n_blocks]: pool slot of column nb's plane, kCovZero or kCovOne
+    const uint32_t* pool;       // [slots][2048]
+};
+
 // One column as the producer warp plans it (every lane holds the same values except the AND-member fields).  With the companion
 // the plan also decides what the consumers would otherwise learn from the column's descriptor row: which streamed stages are
 // AND-group bit-blocks (their stream indices, published sorted), how many there are and the result state.
@@ -1096,10 +1105,14 @@ struct PipeCol {
     const uint8_t *bsrc, *gsrc, *lsrc;
     uint32_t ka, kb;             // stream index of AND member lane / lane + 32 when it is a bit-block, else ~0
     uint32_t ra, rb;             // ... its position in the sorted index list
+    uint32_t rela, relb;         // ... with coverage: its block index in the column's bit segment (streamed in place)
     uint32_t nb0, state;         // AND-group bit-blocks; 0 = NULL, 1 = FULL, 2 = computed (and_state)
 };
 
-__global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(const AggParams p, const RunLists rl)
+// COV: the call streams the coverage plane cv (else cv is null).  A template parameter, so the companion and segment paths compile
+// as they would without it.
+template <bool COV>
+__global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(const AggParams p, const RunLists rl, const Coverage cv)
 {
     constexpr int OP = BMB200_OP_AND_SUB;
     extern __shared__ __align__(128) uint8_t dyn_smem[];
@@ -1125,6 +1138,7 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const uint32_t M = p.set.n_vec;
     const uint32_t n0 = p.goff[1], n1 = p.goff[2] - p.goff[1];
+    const bool planned = COV || rl.sgl_base != nullptr;     // the producer's plan replaces the classification
     if (tid == 0) {
         for (int s = 0; s < kPipeStages; ++s) { mbar_init(&s_full[s], 1u); mbar_init(&s_empty[s], kPipeWarps); }
         for (int q = 0; q < kPipeQueue; ++q) { mbar_init(&s_qfull[q], 1u); mbar_init(&s_qempty[q], kPipeWarps); }
@@ -1133,7 +1147,7 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
     for (uint32_t i = tid; i < kPipeMaxVec / 32; i += kPipeThreads) { s_g1[i] = 0u; s_brole[0][i] = 0u; }
     if (tid < 12) (&s_st[0][0])[tid] = (tid % 6 == 5) ? ~0u : 0u;
     __syncthreads();
-    if (!rl.sgl_base)                                       // the descriptor-row classification's role table
+    if (!planned)                                           // the descriptor-row classification's role table
         for (uint32_t k = n0 + tid; k < n0 + n1; k += kPipeThreads) { const uint32_t v = p.group[k]; atomicOr(&s_g1[v >> 5], 1u << (v & 31u)); }
     __syncthreads();                                        // the last CTA-wide barrier: the producer warp leaves below
 
@@ -1153,6 +1167,27 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
             const uint32_t nbit = (uint32_t)(p.set.bit_base[nb + 1] - b0);
             c.bsrc = reinterpret_cast<const uint8_t*>(p.set.bit_pool + b0 * kBlockWords);
             c.ka = c.kb = ~0u;
+            if (COV) {          // coverage: the AND members' bit-blocks (stream index = rank among them), then the plane
+                const uint32_t* drow = p.set.desc + (size_t)nb * M;
+                const uint32_t da = ma != ~0u ? drow[ma] : 0u, db = mb != ~0u ? drow[mb] : 0u;
+                const uint32_t cs = cv.slot[nb];
+                const bool ba = ma != ~0u && (da & 3u) == BMB200_BLK_BIT, bb = mb != ~0u && (db & 3u) == BMB200_BLK_BIT;
+                const uint32_t mba = __ballot_sync(0xffffffffu, ba), mbb = __ballot_sync(0xffffffffu, bb);
+                const uint32_t null0 = __ballot_sync(0xffffffffu, (ma != ~0u && (da & 3u) == BMB200_BLK_NULL) ||
+                                                                  (mb != ~0u && (db & 3u) == BMB200_BLK_NULL));
+                c.nb0 = __popc(mba) + __popc(mbb);
+                c.state = (null0 || n0 == 0u || cs == kCovOne) ? 0u : (c.nb0 == 0u && n1 == 0u) ? 1u : 2u;
+                if (c.state == 0u) { c.nb0 = 0u; return c; }                 // a NULL result streams nothing
+                const uint32_t lt = (1u << lane) - 1u;
+                if (ba) { c.ka = c.ra = __popc(mba & lt); c.rela = (da >> 2) & kRelMask; }
+                if (bb) { c.kb = c.rb = __popc(mba) + __popc(mbb & lt); c.relb = (db >> 2) & kRelMask; }
+                c.nstr = c.nb0;
+                if (cs != kCovZero) {
+                    c.un = 1u; c.gbytes = kPipeStage;
+                    c.gsrc = reinterpret_cast<const uint8_t*>(cv.pool + (size_t)cs * kBlockWords);
+                }
+                return c;
+            }
             // behind the bit-blocks: the GAP segment (gsrc, gbytes), or the companion's singles (gsrc, gbytes) and long runs (lsrc, lbytes)
             if (rl.sgl_base) {
                 const uint32_t* drow = p.set.desc + (size_t)nb * M;
@@ -1218,7 +1253,7 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
         uint32_t seq = 0;
         for (uint32_t qi = 0;; ++qi) {
             const uint32_t par = qi & 1u, ng = cur.nstr + (cur.gbytes + kPipeStage - 1u) / kPipeStage;
-            const uint32_t ns = ng + (cur.lbytes + kPipeStage - 1u) / kPipeStage, jp = rl.sgl_base ? 0u : max(ns, 1u) - 1u;
+            const uint32_t ns = ng + (cur.lbytes + kPipeStage - 1u) / kPipeStage, jp = planned ? 0u : max(ns, 1u) - 1u;
             PipeCol nxt;
             for (uint32_t j = 0, jb = 0; j < max(ns, 1u); ++j) {
                 if (j < ns) {
@@ -1227,7 +1262,12 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
                         while ((s_lst[par ^ 1u][jb >> 5] >> (jb & 31u)) & 1u) ++jb;
                     mbar_wait(&s_empty[s], ((seq / kPipeStages) & 1u) ^ 1u);
                     uint32_t bytes; const uint8_t* src;
-                    if (j < cur.nstr) { bytes = kPipeStage; src = cur.bsrc + (size_t)jb++ * kPipeStage; }
+                    if (COV && j < cur.nstr) {                   // coverage: AND member with stream index j, in place
+                        const uint32_t ha = __ballot_sync(0xffffffffu, cur.ka == j), hb = __ballot_sync(0xffffffffu, cur.kb == j);
+                        const uint32_t rel = ha ? __shfl_sync(0xffffffffu, cur.rela, __ffs(ha) - 1) : __shfl_sync(0xffffffffu, cur.relb, __ffs(hb) - 1);
+                        bytes = kPipeStage; src = cur.bsrc + (size_t)rel * kPipeStage;
+                    }
+                    else if (j < cur.nstr) { bytes = kPipeStage; src = cur.bsrc + (size_t)jb++ * kPipeStage; }
                     else if (j < ng)  { const uint32_t o = (j - cur.nstr) * kPipeStage; bytes = min(kPipeStage, cur.gbytes - o); src = cur.gsrc + o; }
                     else              { const uint32_t o = (j - ng) * kPipeStage;       bytes = min(kPipeStage, cur.lbytes - o); src = cur.lsrc + o; }
                     if (lane == 0) {
@@ -1262,7 +1302,6 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
     asm volatile("mov.u32 %0, %1;" : "=r"(Ks) : "r"(smem_u32(K)));
     asm volatile("mov.u32 %0, %1;" : "=r"(ring_s) : "r"(smem_u32(ring)));
     constexpr int H = kPipeWpt / 4;
-    const bool planned = rl.sgl_base != nullptr;             // the companion path: the producer's plan replaces the classification
     for (uint32_t qi = 0;; ++qi) {
         const uint32_t b = qi & 1u, qs = qi % kPipeQueue;
         if (!planned) {

@@ -82,10 +82,11 @@ struct bmb200_ctx {
     int gap_mode = 0;                       // 0 = stream sorted GAP lists through the smem ring, 1 = always gather
     bool attr_set = false, merge_attr_set = false;
     size_t agg_dyn[4] = {};                 // dynamic shared memory per agg_kernel<OP> (set_agg_attrs)
-    size_t pipe_dyn = 0;                    // ... of agg_pipe_kernel
+    size_t pipe_dyn[2] = {};                // ... of agg_pipe_kernel<COV> (the static part differs), by COV
     int pipe_ctas_per_sm = 1;               // resident agg_pipe_kernel CTAs per SM with that shared memory (occupancy query)
     int agg_pipeline = 1;                   // 1 = whole-set AND-SUB takes agg_pipe_kernel, 0 = always agg_kernel
     int run_lists = 1;                      // run-list companion of agg_pipe_kernel: 0 never, 1 from a set's second qualifying call, 2 from its first
+    int coverage = 1;                       // coverage planes of agg_pipe_kernel: 0 never, 1 from a set's third qualifying call with that n0, 2 from its first
     int host_threads = 0;                   // host threads of bmb200_set_upload_vectors (0 = hardware concurrency, at most 64)
     uint8_t* h_ring[kStageSlots] = {};      // pinned staging ring of bmb200_set_upload_vectors (grow-only)
     size_t h_ring_cap = 0;
@@ -128,6 +129,17 @@ struct bmb200_set {
     uint32_t* rl_un_pool = nullptr;         // [slots][2048]
     uint16_t* rl_full = nullptr;            // [n_blocks]: FULL blocks per column
     uint64_t rl_un_a = 0, rl_un_ab = 0;     // columns that stream U_A / U_AB (bmb200_set_run_list_unions)
+    // coverage planes GT_n0 (coverage_kernel.cuh), one per AND-group size n0 in the order the sizes first qualify, at most
+    // kCovMaxPlanes and never evicted; always owned by the set and freed with it
+    struct CovPlane {
+        uint32_t n0 = 0;
+        int state = 0;                      // 0 not built, 1 built, -1 cannot be built (device memory): calls run without it
+        uint32_t calls = 0;                 // qualifying calls seen while not built
+        uint32_t* slot = nullptr;           // [n_blocks]: pool slot, kCovZero or kCovOne
+        uint32_t* pool = nullptr;           // [stored][2048]
+        uint64_t stored = 0, one = 0;       // columns with a stored plane, kCovOne columns (bmb200_set_coverage)
+    };
+    std::vector<CovPlane> cov;
     size_t cap_desc = 0, cap_base = 0, cap_bit = 0, cap_gap = 0;   // capacities when the arrays came from set_alloc (elements / blocks / units); 0 = not recyclable
 };
 
@@ -234,6 +246,12 @@ void free_run_lists(bmb200_set* s)
     s->rl_sgl_units = s->rl_lr_units = s->rl_b_sgl_units = s->rl_b_lr_units = s->rl_listed_blocks = 0;
     s->rl_sgl_word_units = s->rl_b_sgl_word_units = 0;
     s->listed_vecs.clear();
+}
+
+void free_coverage(bmb200_set* s)
+{
+    for (auto& c : s->cov) { cudaFree(c.slot); cudaFree(c.pool); }
+    s->cov.clear();
 }
 
 void free_result_arrays(bmb200_result* r)
@@ -413,6 +431,7 @@ int bmb200_ctx_set_tuning(bmb200_ctx* ctx, int key, int value)
     if (key == BMB200_TUNE_HOST_THREADS && value >= 0 && value <= 64) { ctx->host_threads = value; return BMB200_OK; }
     if (key == BMB200_TUNE_AGG_PIPELINE && (value == 0 || value == 1)) { ctx->agg_pipeline = value; return BMB200_OK; }
     if (key == BMB200_TUNE_RUN_LISTS && value >= 0 && value <= 2) { ctx->run_lists = value; return BMB200_OK; }
+    if (key == BMB200_TUNE_COVERAGE && value >= 0 && value <= 2) { ctx->coverage = value; return BMB200_OK; }
     return BMB200_ERR_BADARG;
 }
 
@@ -1092,6 +1111,7 @@ int bmb200_set_free(bmb200_set* s)
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
     free_run_lists(s);                                       // derived data: never parked
+    free_coverage(s);
     if (s->owns && s->cap_desc && !ctx->arena.full) {       // park the arrays for the next upload instead of cudaFree
         auto& a = ctx->arena;
         a.desc = (void*)s->v.desc; a.bb = (void*)s->v.bit_base; a.gb = (void*)s->v.gap_base; a.bp = (void*)s->v.bit_pool; a.gp = (void*)s->v.gap_pool;
@@ -1229,10 +1249,11 @@ static void set_agg_attrs(bmb200_ctx* ctx, cudaError_t* e)
     if (cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, ctx->device) != cudaSuccess) { cudaGetLastError(); reserved = 1024; }
     *e = cudaSuccess;
     for (int op = 0; op < 4 && *e == cudaSuccess; ++op) *e = agg_attr_one(kAggKernels[op], (size_t)reserved, &ctx->agg_dyn[op]);
-    if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel, (size_t)reserved, &ctx->pipe_dyn, kPipeRingSmem);
+    if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel<false>, (size_t)reserved, &ctx->pipe_dyn[0], kPipeRingSmem);
+    if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel<true>, (size_t)reserved, &ctx->pipe_dyn[1], kPipeRingSmem);
     // the kernel is shaped for kPipeCtasPerSm CTAs per SM; its grid follows what the device actually grants (at least one)
     if (*e == cudaSuccess)
-        *e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->pipe_ctas_per_sm, agg_pipe_kernel, (int)kPipeThreads, ctx->pipe_dyn);
+        *e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->pipe_ctas_per_sm, agg_pipe_kernel<false>, (int)kPipeThreads, ctx->pipe_dyn[0]);
     if (*e == cudaSuccess && ctx->pipe_ctas_per_sm < 1) ctx->pipe_ctas_per_sm = 1;
     if (*e == cudaSuccess) ctx->attr_set = true;
 }
@@ -1441,6 +1462,68 @@ static bool use_run_lists(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_b
     return true;
 }
 
+// Builds the coverage plane of c.n0 (coverage_kernel.cuh): one CTA per column into a pool with a slot for every column, one wait
+// for the number of stored columns, then a copy into a pool of that size.  On any failure, or when the worst-case pool would leave
+// less than kRunListMargin of device memory free, this n0 is marked as having none (state = -1).
+constexpr size_t kCovMaxPlanes = 4;
+static bool build_coverage(bmb200_ctx* ctx, bmb200_set* s, bmb200_set::CovPlane& c)
+{
+    const uint32_t nb = s->v.n_blocks;
+    cudaStream_t st = ctx->stream;
+    uint32_t* tmp = nullptr; unsigned long long* tot = nullptr;
+    uint64_t h_tot[2] = {0, 0};
+    size_t free_b = 0, total_b = 0;
+    bool ok = cudaMemGetInfo(&free_b, &total_b) == cudaSuccess && free_b >= (size_t)nb * (kPipeStage + 4u) + kRunListMargin &&
+              cudaMalloc((void**)&c.slot, (size_t)nb * 4u) == cudaSuccess && cudaMalloc((void**)&tmp, (size_t)nb * kPipeStage) == cudaSuccess &&
+              cudaMalloc((void**)&tot, sizeof(h_tot)) == cudaSuccess && cudaMemsetAsync(tot, 0, sizeof(h_tot), st) == cudaSuccess &&
+              cudaFuncSetAttribute(cov_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCovSmem) == cudaSuccess;
+    if (ok) {
+        cov_kernel<<<nb, kRlThreads, kCovSmem, st>>>(s->v, c.n0, c.slot, tmp, tot);
+        ok = cudaGetLastError() == cudaSuccess && cudaMemcpyAsync(h_tot, tot, sizeof(h_tot), cudaMemcpyDeviceToHost, st) == cudaSuccess &&
+             cudaStreamSynchronize(st) == cudaSuccess;
+    }
+    ok = ok && cudaMalloc((void**)&c.pool, std::max<uint64_t>(h_tot[0], 1u) * kPipeStage) == cudaSuccess &&
+         cudaMemcpyAsync(c.pool, tmp, h_tot[0] * kPipeStage, cudaMemcpyDeviceToDevice, st) == cudaSuccess &&
+         cudaStreamSynchronize(st) == cudaSuccess;
+    cudaFree(tmp); cudaFree(tot);
+    if (!ok) { cudaGetLastError(); cudaFree(c.slot); cudaFree(c.pool); c.slot = c.pool = nullptr; c.state = -1; return false; }
+    c.stored = h_tot[0]; c.one = h_tot[1]; c.state = 1;
+    return true;
+}
+
+// agg_pipe_kernel streams the AND-group bit-blocks and the coverage plane of n0 = |AND group| when no AND-group member holds a GAP
+// block anywhere in the set (the plane holds every SUB-group block, bit-blocks listed or not, and the AND members' FULL blocks).
+// Builds the plane when due (ctx->coverage; by default on the third call, so the companion's default rule still builds it on the
+// second and a one-shot set builds neither); false = the call runs without it.
+static bool use_coverage(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_batch_args* a, Coverage* cv)
+{
+    bmb200_set* s = const_cast<bmb200_set*>(set);
+    const uint32_t n0 = a->offsets[1] - a->offsets[0];
+    if (!ctx->coverage || n0 == 0) return false;
+    const std::vector<uint32_t>& gv = gap_vectors(ctx, set);
+    if (gv.empty()) return false;
+    for (uint32_t k = a->offsets[0]; k < a->offsets[1]; ++k)
+        if ((gv[a->members[k] >> 5] >> (a->members[k] & 31u)) & 1u) return false;
+    auto c = std::find_if(s->cov.begin(), s->cov.end(), [&](const bmb200_set::CovPlane& x) { return x.n0 == n0; });
+    if (c == s->cov.end()) {
+        if (s->cov.size() >= kCovMaxPlanes) return false;
+        s->cov.emplace_back(); s->cov.back().n0 = n0; c = s->cov.end() - 1;
+    }
+    if (c->state < 0) return false;
+    if (c->state == 0 && (++c->calls < (ctx->coverage == 1 ? 3u : 1u) || !build_coverage(ctx, s, *c))) return false;
+    *cv = Coverage{c->slot, c->pool};
+    return true;
+}
+
+int bmb200_set_coverage(const bmb200_set* s, uint32_t n0, uint64_t* stored_cols, uint64_t* one_cols)
+{
+    if (!s || !stored_cols || !one_cols) return BMB200_ERR_BADARG;
+    *stored_cols = *one_cols = 0;
+    for (const auto& c : s->cov)
+        if (c.n0 == n0 && c.state == 1) { *stored_cols = c.stored; *one_cols = c.one; }
+    return BMB200_OK;
+}
+
 int bmb200_set_run_list_unions(const bmb200_set* s, uint64_t* a_cols, uint64_t* ab_cols)
 {
     if (!s || !a_cols || !ab_cols) return BMB200_ERR_BADARG;
@@ -1526,15 +1609,19 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     uint32_t grid = sms * (uint32_t)ctx->agg_ctas_per_sm;
     if (grid > n_cols) grid = n_cols;
     RunLists rl{};
+    Coverage cv{};
     if (ctx->agg_pipeline && ctx->gap_mode == 0 && set->n_gap_units && whole_set(a, set->v.n_vec) &&
-        (use_run_lists(ctx, set, a, &rl) || flat_gap_set(ctx, set))) {
+        (use_coverage(ctx, set, a, &cv) || use_run_lists(ctx, set, a, &rl) || flat_gap_set(ctx, set))) {
         // one AND-SUB group naming every vector once: a producer warp per CTA streams whole columns (agg_pipe_kernel), two CTAs
-        // per SM, with the GAP segments or the run-list companion behind the bit-blocks.
+        // per SM: the AND-group bit-blocks and the coverage plane, or every bit-block with the GAP segments or the run-list
+        // companion behind them.
         // OR stays on agg_kernel: its whole-set workloads measured at par or slower through the ring (DESIGN §3.1a)
-        p.dyn_bytes = (uint32_t)ctx->pipe_dyn;
+        const bool cov = cv.slot != nullptr;
+        p.dyn_bytes = (uint32_t)ctx->pipe_dyn[cov];
         const uint32_t pctas = sms * (uint32_t)ctx->pipe_ctas_per_sm;
         const uint32_t pgrid = pctas < n_cols ? pctas : n_cols;
-        agg_pipe_kernel<<<pgrid, kPipeThreads, ctx->pipe_dyn, ctx->stream>>>(p, rl);
+        if (cov) agg_pipe_kernel<true><<<pgrid, kPipeThreads, ctx->pipe_dyn[1], ctx->stream>>>(p, rl, cv);
+        else agg_pipe_kernel<false><<<pgrid, kPipeThreads, ctx->pipe_dyn[0], ctx->stream>>>(p, rl, cv);
     } else if (a->op == BMB200_OP_SHIFT_R_AND) {
         shift_and_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p);
     } else {

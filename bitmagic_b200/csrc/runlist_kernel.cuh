@@ -76,23 +76,32 @@ struct SglOut {
     }
 };
 
-// One warp decodes the GAP block at g (= &buf[0], lead pad already skipped): singles through so, long-run pairs in order to
-// lout[nl..) unless lout is null.  ns / nl are warp-uniform running counts.
+// The GAP block at g (= &buf[0], lead pad already skipped) with header hdr = g[0] holds gap_ones(hdr) 1-runs; gap_one_run gives
+// 1-run j as bits [s, e] (run k = 2j+1 when the first run is 1, else 2j+2).
+__device__ __forceinline__ uint32_t gap_ones(uint32_t hdr)
+{
+    const uint32_t len = hdr >> 3;
+    return (hdr & 1u) ? (len + 1u) >> 1 : len >> 1;
+}
+__device__ __forceinline__ void gap_one_run(const uint16_t* __restrict__ g, uint32_t hdr, uint32_t j, uint32_t& s, uint32_t& e)
+{
+    const uint32_t k = 2u * j + ((hdr & 1u) ? 1u : 2u);
+    s = (k == 1u) ? 0u : g[k - 1u] + 1u;
+    e = g[k];
+}
+
+// One warp decodes the GAP block at g: singles through so, long-run pairs in order to lout[nl..) unless lout is null.  ns / nl
+// are warp-uniform running counts.
 __device__ __forceinline__ void rl_block(const uint16_t* __restrict__ g, uint32_t lane, uint32_t& ns, uint32_t& nl,
                                          const SglOut& so, uint32_t* lout)
 {
-    const uint32_t hdr = g[0], len = hdr >> 3, first = hdr & 1u;
-    const uint32_t nsel = first ? (len + 1u) >> 1 : len >> 1;      // 1-runs: k = 2j+1 (first run is 1) or 2j+2
+    const uint32_t hdr = g[0], nsel = gap_ones(hdr);
     const uint32_t lt = (1u << lane) - 1u;
     for (uint32_t j0 = 0; j0 < nsel; j0 += 32u) {
         const uint32_t j = j0 + lane;
         uint32_t s = 0, e = 0;
         const bool ok = j < nsel;
-        if (ok) {
-            const uint32_t k = 2u * j + (first ? 1u : 2u);
-            s = (k == 1u) ? 0u : g[k - 1u] + 1u;
-            e = g[k];
-        }
+        if (ok) gap_one_run(g, hdr, j, s, e);
         const bool sg = ok && (s == e || s == 0u), lg = ok && e > s;
         const uint32_t bs = __ballot_sync(0xffffffffu, sg), bl = __ballot_sync(0xffffffffu, lg);
         if (sg) so.put(s);
@@ -101,10 +110,10 @@ __device__ __forceinline__ void rl_block(const uint16_t* __restrict__ g, uint32_
     }
 }
 
-// Warp w of a column takes vectors [w * per, (w + 1) * per): its long runs land in vector order behind those of warps < w.
-// nfull (unless null) grows by the warp's FULL blocks.
-__device__ __forceinline__ void rl_column(const SetView v, uint32_t nb, uint32_t warp, uint32_t lane, uint32_t& ns, uint32_t& nl,
-                                          const SglOut& so, uint32_t* lout, uint32_t* nfull = nullptr)
+// Warp w of a column takes vectors [w * per, (w + 1) * per) and hands each GAP block, in vector order, to blk(g) (g = &buf[0],
+// lead pad skipped) with the whole warp.  nfull (unless null) grows by the warp's FULL blocks.
+template <typename F>
+__device__ __forceinline__ void rl_gap_blocks(const SetView v, uint32_t nb, uint32_t warp, uint32_t lane, uint32_t* nfull, F&& blk)
 {
     const uint32_t M = v.n_vec, per = (M + kRlWarps - 1u) / kRlWarps;
     const uint32_t* drow = v.desc + (size_t)nb * M;
@@ -117,9 +126,16 @@ __device__ __forceinline__ void rl_column(const SetView v, uint32_t nb, uint32_t
         while (m) {
             const int l = __ffs(m) - 1; m &= m - 1u;
             const uint32_t dl = __shfl_sync(0xffffffffu, d, l);
-            rl_block(gseg + (size_t)((dl >> 2) & BMB200_DESC_REL_MASK) * kGapUnit + (dl >> 31), lane, ns, nl, so, lout);
+            blk(gseg + (size_t)((dl >> 2) & BMB200_DESC_REL_MASK) * kGapUnit + (dl >> 31));
         }
     }
+}
+
+// The column's GAP blocks through rl_block: warp w's long runs land in vector order behind those of warps < w.
+__device__ __forceinline__ void rl_column(const SetView v, uint32_t nb, uint32_t warp, uint32_t lane, uint32_t& ns, uint32_t& nl,
+                                          const SglOut& so, uint32_t* lout, uint32_t* nfull = nullptr)
+{
+    rl_gap_blocks(v, nb, warp, lane, nfull, [&](const uint16_t* g) { rl_block(g, lane, ns, nl, so, lout); });
 }
 
 __device__ __forceinline__ uint32_t warp_excl_scan(uint32_t v, uint32_t lane, uint32_t& total)

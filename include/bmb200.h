@@ -197,6 +197,11 @@ int bmb200_device_info(const bmb200_ctx* ctx, int* sm_count, int* cc_major, int*
 #define BMB200_TUNE_AGG_PIPELINE 3   /* 1 (default) = whole-set AND-SUB aggregations take the streamed-column kernel, 0 = never (A/B reference) */
 #define BMB200_TUNE_RUN_LISTS    4   /* run-list companion of a set's GAP blocks, streamed by the whole-set AND-SUB kernel when the AND group
                                         holds no GAP block: 1 (default) = built on the set's second such call, 2 = on its first, 0 = never */
+#define BMB200_TUNE_COVERAGE     5   /* coverage plane of a set per AND-group size n0 (the bits more than n0 vectors hold), streamed by the
+                                        whole-set AND-SUB kernel in place of the SUB group when the AND group holds no GAP block: 1
+                                        (default) = built on the set's third such call with that n0 (the companion's default still
+                                        builds on the second), 2 = on its first, 0 = never.  At most 4 sizes per set; once built it
+                                        is preferred over the run-list companion */
 int bmb200_ctx_set_tuning(bmb200_ctx* ctx, int key, int value);
 /* pin the CALLING thread (and the threads it starts later, e.g. the packers of bmb200_set_upload_vectors) to the CPUs of the NUMA
  * node this context's GPU hangs off, so that pinned staging memory is allocated next to the GPU's PCIe root.  *node = the node, or
@@ -279,6 +284,9 @@ int bmb200_set_packed_singles(const bmb200_set* set, uint64_t* a_bytes, uint64_t
 /* how many columns stream part A, and parts A + B, of the companion as one 8 KB union mask (the bits the part's runs cover) in
  * place of the packed part: those whose part takes 8192 bytes or more as streamed; 0 / 0 while none is built. */
 int bmb200_set_run_list_unions(const bmb200_set* set, uint64_t* a_cols, uint64_t* ab_cols);
+/* the set's coverage plane of AND-group size n0 (BMB200_TUNE_COVERAGE): how many columns store an 8 KB plane, and how many are
+ * covered everywhere (their AND-SUB result is empty); 0 / 0 while none is built.  The planes are freed with the set. */
+int bmb200_set_coverage(const bmb200_set* set, uint32_t n0, uint64_t* stored_cols, uint64_t* one_cols);
 
 /* synthetic input generator (bench / test support): vector v has iid bit density
  * density[v], counter-based RNG keyed by seed[v]; with optimize != 0 every block is

@@ -71,7 +71,7 @@ if not args.no_run_lists:
         for l in run(lib, ["scripts/bench_run_lists.py"]):
             print(json.dumps({"lib": i, "bench_run_lists": l}), flush=True)
             if l.get("and_group") == [1, 2]:
-                streamed[i] = l["streamed_bytes_mode1"]
+                streamed[i] = l.get("streamed_bytes", l["streamed_bytes_mode1"])   # what the default path streams
 
 summary = {"card": card, "dumps_identical": same}
 for wl in ms:
