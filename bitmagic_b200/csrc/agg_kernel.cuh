@@ -1057,8 +1057,13 @@ constexpr uint32_t kPipeMaxVec  = 4096u;                   // role table size: l
 constexpr int      kPipePerThr  = (int)kPipeMaxVec / kPipeConsumers;
 constexpr uint32_t kPipeMaxAndGap = 64u;                   // AND-group GAP blocks per column the FLAT path takes (more: in-place reads)
 constexpr uint32_t kPipeThreads = kPipeConsumers + 32u;    // 8 consumer warps + 1 producer warp
-constexpr size_t   kPipeRingSmem = (size_t)kPipeStages * kPipeStage;
 static_assert(kPipeStages % kPipeGroups == 0, "a ring slot must go to the same warp group each time a column reuses it");
+// The coverage instantiation streams bit stages only (every warp waits for every stage, so any ring depth keeps the parity waits
+// sound) and at most n0 + 1 of them per column (3 on C3).  A shallower ring lets a third CTA per SM keep one more column's
+// fixed per-column work (queue hand-off, fold, finish_block) in flight; at three CTAs the register cap is 72.
+constexpr int      kCovCtasPerSm = 3;
+constexpr int      kCovStages    = 6;
+constexpr size_t pipe_ring_smem(bool cov) { return (size_t)(cov ? kCovStages : kPipeStages) * kPipeStage; }
 static_assert(kPipeWpt == 8 && kPipeStage == 2u * 16u * kPipeConsumers, "a bit stage is two LDS.128 per consumer thread");
 
 // *bad |= 1 when a GAP block of the set is not in the BMB200_DESC_GAP_FLAT form (agg_pipe_kernel sweeps SUB-group blocks as FLAT pairs)
@@ -1112,17 +1117,18 @@ struct PipeCol {
 // COV: the call streams the coverage plane cv (else cv is null).  A template parameter, so the companion and segment paths compile
 // as they would without it.
 template <bool COV>
-__global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(const AggParams p, const RunLists rl, const Coverage cv)
+__global__ void __launch_bounds__(kPipeThreads, COV ? kCovCtasPerSm : kPipeCtasPerSm) agg_pipe_kernel(const AggParams p, const RunLists rl, const Coverage cv)
 {
     constexpr int OP = BMB200_OP_AND_SUB;
+    constexpr int NS = COV ? kCovStages : kPipeStages;    // ring stages
     extern __shared__ __align__(128) uint8_t dyn_smem[];
     const uint32_t dyn_s = smem_u32(dyn_smem);
     const uint32_t k_off = ((dyn_s + kLiveAlign - 1u) & ~(kLiveAlign - 1u)) - dyn_s;
-    if (k_off + kLiveAlign + (uint32_t)kPipeRingSmem > p.dyn_bytes) __trap();     // host and kernel disagree about the layout
+    if (k_off + kLiveAlign + (uint32_t)NS * kPipeStage > p.dyn_bytes) __trap();     // host and kernel disagree about the layout
     uint32_t* K = reinterpret_cast<uint32_t*>(dyn_smem + k_off);
     uint8_t* ring = dyn_smem + k_off + kLiveAlign;
 
-    __shared__ __align__(8) uint64_t s_full[kPipeStages], s_empty[kPipeStages], s_qfull[kPipeQueue], s_qempty[kPipeQueue];
+    __shared__ __align__(8) uint64_t s_full[NS], s_empty[NS], s_qfull[kPipeQueue], s_qempty[kPipeQueue];
     __shared__ uint4 s_q[kPipeQueue];                       // (item | ~0 = end, bit stages, GAP or companion singles bytes, first stage)
     __shared__ uint32_t s_qlr[kPipeQueue];                  // companion long-run bytes (0 without the companion)
     __shared__ uint32_t s_qpl[kPipeQueue];                  // companion plan: AND-group bit-blocks | result state << 16
@@ -1140,7 +1146,7 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
     const uint32_t n0 = p.goff[1], n1 = p.goff[2] - p.goff[1];
     const bool planned = COV || rl.sgl_base != nullptr;     // the producer's plan replaces the classification
     if (tid == 0) {
-        for (int s = 0; s < kPipeStages; ++s) { mbar_init(&s_full[s], 1u); mbar_init(&s_empty[s], kPipeWarps); }
+        for (int s = 0; s < NS; ++s) { mbar_init(&s_full[s], 1u); mbar_init(&s_empty[s], kPipeWarps); }
         for (int q = 0; q < kPipeQueue; ++q) { mbar_init(&s_qfull[q], 1u); mbar_init(&s_qempty[q], kPipeWarps); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
@@ -1257,10 +1263,10 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
             PipeCol nxt;
             for (uint32_t j = 0, jb = 0; j < max(ns, 1u); ++j) {
                 if (j < ns) {
-                    const uint32_t s = seq % kPipeStages;
+                    const uint32_t s = seq % NS;
                     if (j < cur.nstr && cur.nlst)                // the next unlisted bit-block
                         while ((s_lst[par ^ 1u][jb >> 5] >> (jb & 31u)) & 1u) ++jb;
-                    mbar_wait(&s_empty[s], ((seq / kPipeStages) & 1u) ^ 1u);
+                    mbar_wait(&s_empty[s], ((seq / NS) & 1u) ^ 1u);
                     uint32_t bytes; const uint8_t* src;
                     if (COV && j < cur.nstr) {                   // coverage: AND member with stream index j, in place
                         const uint32_t ha = __ballot_sync(0xffffffffu, cur.ka == j), hb = __ballot_sync(0xffffffffu, cur.kb == j);
@@ -1392,8 +1398,8 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
         for (int h = 0; h < H; ++h) { acc0[h] = make_uint4(~0u, ~0u, ~0u, ~0u); acc1[h] = make_uint4(0u, 0u, 0u, 0u); }
         uint32_t na = 0, and_j = __shfl_sync(0xffffffffu, ia, 0);
         for (uint32_t j = 0; j < nbit; ++j) {
-            const uint32_t sq = seq0 + j, s = sq % kPipeStages;
-            mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
+            const uint32_t sq = seq0 + j, s = sq % NS;
+            mbar_wait(&s_full[s], (sq / NS) & 1u);
             uint4 v[H];
 #pragma unroll
             for (int h = 0; h < H; ++h) v[h] = lds128(ring_s + s * kPipeStage + (uint32_t)(h * kPipeConsumers + tid) * 16u);
@@ -1433,11 +1439,11 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
             // and long runs (the stages behind them) from L; no lead-pad repair, no AND-group blocks
             uint32_t flat_mode = 0;
             for (uint32_t g = grp; g < nst; g += kPipeGroups) {
-                const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
+                const uint32_t sq = seq0 + nbit + g, s = sq % NS;
                 const bool sgl = g < ngs;
                 const uint32_t bytes = sgl ? min(kPipeStage, gbytes - g * kPipeStage) : min(kPipeStage, lbytes - (g - ngs) * kPipeStage);
                 const uint32_t src = ring_s + s * kPipeStage + wlo + (uint32_t)lane * 16u, sb = bytes > wlo ? bytes - wlo : 0u;
-                mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
+                mbar_wait(&s_full[s], (sq / NS) & 1u);
                 if (sgl) {
                     sgl_sweep_fn(Ks, src, min(kPipeSlice, sb), (uint32_t)lane * 16u);                      // a partial last stage
                 } else {                                                                                   // leaves later slices empty
@@ -1459,9 +1465,9 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
             }
             uint32_t flat_mode = 0;
             for (uint32_t g = grp; g < ngs; g += kPipeGroups) {
-                const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
+                const uint32_t sq = seq0 + nbit + g, s = sq % NS;
                 const uint32_t st0 = g * kPipeStage, bytes = min(kPipeStage, gbytes - st0), sb = bytes > wlo ? bytes - wlo : 0u;
-                mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
+                mbar_wait(&s_full[s], (sq / NS) & 1u);
                 if (nag) {   // blank the AND-group bytes of this warp's slice: as zero pairs the sweep reads no run in them
                     const uint32_t w0 = st0 + wlo, w1 = w0 + min(kPipeSlice, sb);
                     for (uint32_t i = 0; i < nag; ++i) {
@@ -1480,8 +1486,8 @@ __global__ void __launch_bounds__(kPipeThreads, kPipeCtasPerSm) agg_pipe_kernel(
             }
         } else {
             for (uint32_t g = 0; g < ngs; ++g) {                      // release the staged segment unread
-                const uint32_t sq = seq0 + nbit + g, s = sq % kPipeStages;
-                mbar_wait(&s_full[s], (sq / kPipeStages) & 1u);
+                const uint32_t sq = seq0 + nbit + g, s = sq % NS;
+                mbar_wait(&s_full[s], (sq / NS) & 1u);
                 if (lane == 0) mbar_arrive(&s_empty[s]);
             }
             for (int i = 0; i < kPipePerThr; ++i) {                   // this warp's 32 vectors of trip i, one GAP block at a time

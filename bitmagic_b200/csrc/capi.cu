@@ -83,7 +83,7 @@ struct bmb200_ctx {
     bool attr_set = false, merge_attr_set = false;
     size_t agg_dyn[4] = {};                 // dynamic shared memory per agg_kernel<OP> (set_agg_attrs)
     size_t pipe_dyn[2] = {};                // ... of agg_pipe_kernel<COV> (the static part differs), by COV
-    int pipe_ctas_per_sm = 1;               // resident agg_pipe_kernel CTAs per SM with that shared memory (occupancy query)
+    int pipe_ctas_per_sm[2] = {1, 1};       // resident agg_pipe_kernel<COV> CTAs per SM with that shared memory (occupancy query)
     int agg_pipeline = 1;                   // 1 = whole-set AND-SUB takes agg_pipe_kernel, 0 = always agg_kernel
     int run_lists = 1;                      // run-list companion of agg_pipe_kernel: 0 never, 1 from a set's second qualifying call, 2 from its first
     int coverage = 1;                       // coverage planes of agg_pipe_kernel: 0 never, 1 from a set's third qualifying call with that n0, 2 from its first
@@ -1249,12 +1249,15 @@ static void set_agg_attrs(bmb200_ctx* ctx, cudaError_t* e)
     if (cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, ctx->device) != cudaSuccess) { cudaGetLastError(); reserved = 1024; }
     *e = cudaSuccess;
     for (int op = 0; op < 4 && *e == cudaSuccess; ++op) *e = agg_attr_one(kAggKernels[op], (size_t)reserved, &ctx->agg_dyn[op]);
-    if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel<false>, (size_t)reserved, &ctx->pipe_dyn[0], kPipeRingSmem);
-    if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel<true>, (size_t)reserved, &ctx->pipe_dyn[1], kPipeRingSmem);
-    // the kernel is shaped for kPipeCtasPerSm CTAs per SM; its grid follows what the device actually grants (at least one)
+    if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel<false>, (size_t)reserved, &ctx->pipe_dyn[0], pipe_ring_smem(false));
+    if (*e == cudaSuccess) *e = agg_attr_one(agg_pipe_kernel<true>, (size_t)reserved, &ctx->pipe_dyn[1], pipe_ring_smem(true));
+    // the kernel is shaped for kPipeCtasPerSm CTAs per SM (kCovCtasPerSm with the coverage plane); its grid follows what the
+    // device actually grants (at least one)
     if (*e == cudaSuccess)
-        *e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->pipe_ctas_per_sm, agg_pipe_kernel<false>, (int)kPipeThreads, ctx->pipe_dyn[0]);
-    if (*e == cudaSuccess && ctx->pipe_ctas_per_sm < 1) ctx->pipe_ctas_per_sm = 1;
+        *e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->pipe_ctas_per_sm[0], agg_pipe_kernel<false>, (int)kPipeThreads, ctx->pipe_dyn[0]);
+    if (*e == cudaSuccess)
+        *e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctx->pipe_ctas_per_sm[1], agg_pipe_kernel<true>, (int)kPipeThreads, ctx->pipe_dyn[1]);
+    for (int c = 0; c < 2; ++c) if (*e == cudaSuccess && ctx->pipe_ctas_per_sm[c] < 1) ctx->pipe_ctas_per_sm[c] = 1;
     if (*e == cudaSuccess) ctx->attr_set = true;
 }
 
@@ -1618,7 +1621,7 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
         // OR stays on agg_kernel: its whole-set workloads measured at par or slower through the ring (DESIGN §3.1a)
         const bool cov = cv.slot != nullptr;
         p.dyn_bytes = (uint32_t)ctx->pipe_dyn[cov];
-        const uint32_t pctas = sms * (uint32_t)ctx->pipe_ctas_per_sm;
+        const uint32_t pctas = sms * (uint32_t)ctx->pipe_ctas_per_sm[cov];
         const uint32_t pgrid = pctas < n_cols ? pctas : n_cols;
         if (cov) agg_pipe_kernel<true><<<pgrid, kPipeThreads, ctx->pipe_dyn[1], ctx->stream>>>(p, rl, cv);
         else agg_pipe_kernel<false><<<pgrid, kPipeThreads, ctx->pipe_dyn[0], ctx->stream>>>(p, rl, cv);
