@@ -109,6 +109,8 @@ class ScanStrArgsC(C.Structure):
 
 SCAN_EQ, SCAN_GT, SCAN_GE, SCAN_LT, SCAN_LE, SCAN_RANGE = range(6)
 SCAN_RANGE_OPEN = 6           # lo < element < hi (find_range_float_unbounded); F_FLOAT only
+SCAN_IN = 7                   # element in a list of values (iterator find_eq): one list, one result group
+SCAN_IN_MAX_VALUES = 1 << 20  # longest SCAN_IN list (before de-duplication)
 NO_UNIVERSE = 0xFFFFFFFF
 
 
@@ -580,7 +582,8 @@ def aggregate_batch(ctx: Context, dset: DeviceSet, op: int, groups, flags: int =
 def scan(ctx: Context, dset: DeviceSet, pred: int, values, plane0: int, n_planes: int, universe: int = NO_UNIVERSE,
          flags: int = 0, nb_from: int = 0, nb_to: int = 0, result: DeviceResult | None = None) -> DeviceResult:
     """bmb200_scan: bit-sliced comparison of the sparse vector whose plane j is set vector plane0 + j against every search
-    value (SCAN_RANGE / SCAN_RANGE_OPEN: rows of (lo, hi)); the result has n_values * n_cols columns, value-major.  With
+    value (SCAN_RANGE / SCAN_RANGE_OPEN: rows of (lo, hi)); the result has n_values * n_cols columns, value-major.  SCAN_IN
+    takes the values as one 1-D list and answers the elements equal to any of them in one group of n_cols columns.  With
     F_SIGNED in flags the values are signed (int64) and plane0 is the sign plane of s2u-encoded elements; with F_FLOAT they
     are float32 (their bits are passed, so NaN payloads and -0 keep their meaning) and plane0 is the sign plane of a float vector."""
     if int(flags) & F_FLOAT:
@@ -593,10 +596,12 @@ def scan(ctx: Context, dset: DeviceSet, pred: int, values, plane0: int, n_planes
     nv = vals.shape[0] if two else vals.size
     if two and (vals.ndim != 2 or vals.shape[1] != 2):
         raise ValueError("SCAN_RANGE / SCAN_RANGE_OPEN take an array of (lo, hi) rows")
+    if pred == SCAN_IN and vals.ndim != 1:
+        raise ValueError("SCAN_IN takes one 1-D list of values")
     args = ScanArgsC(int(plane0), int(n_planes), int(universe), int(pred), int(flags), ptr(vals), int(nv), int(nb_from), int(nb_to))
     res = result if result is not None else DeviceResult(ctx)
     ctx.check(lib().bmb200_scan(ctx._h, dset._h, C.byref(args), C.byref(res._h)), "scan")
-    res.n_cols = ((nb_to if nb_to else dset.n_blocks) - nb_from) * int(nv)
+    res.n_cols = ((nb_to if nb_to else dset.n_blocks) - nb_from) * (1 if pred == SCAN_IN else int(nv))
     return res
 
 

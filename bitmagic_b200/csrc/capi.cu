@@ -12,6 +12,7 @@
 #include "aux_kernels.cuh"
 #include "runlist_kernel.cuh"
 #include "scan_kernel.cuh"
+#include "scan_in_kernel.cuh"
 #include "str_scan_kernel.cuh"
 #include "rank_kernel.cuh"
 #include "shift_kernel.cuh"
@@ -50,6 +51,7 @@ enum DevSlot {
     kDevBlobSegs, kDevBlobSegCap,     //   pass 1: segments, their token capacities and processing order
     kDevBlobRecs, kDevBlobERecs,      //   decode records: explicit-length tokens, entropy-coded tokens
     kDevBlobDur,                      //   pass 2: clocks per work item (BMB200_TRACE)
+    kDevScanIn,                       // bmb200_scan BMB200_SCAN_IN: the sorted, unique code list
     kDevSlots
 };
 enum HostSlot {
@@ -80,7 +82,7 @@ struct bmb200_ctx {
     bmb200_set* host_set = nullptr;         // device arena kept between bmb200_aggregate_host calls (cudaMalloc/cudaFree
     bmb200_result* host_res = nullptr;      //   of a multi-GB arena costs tens of ms per call otherwise)
     int gap_mode = 0;                       // 0 = stream sorted GAP lists through the smem ring, 1 = always gather
-    bool attr_set = false, merge_attr_set = false;
+    bool attr_set = false, merge_attr_set = false, scan_in_attr_set = false;
     size_t agg_dyn[4] = {};                 // dynamic shared memory per agg_kernel<OP> (set_agg_attrs)
     size_t pipe_dyn[2] = {};                // ... of agg_pipe_kernel<COV> (the static part differs), by COV
     int pipe_ctas_per_sm[2] = {1, 1};       // resident agg_pipe_kernel<COV> CTAs per SM with that shared memory (occupancy query)
@@ -1694,9 +1696,82 @@ int bmb200_binop(bmb200_ctx* ctx, const bmb200_set* set, int op, uint32_t va, ui
     return BMB200_OK;
 }
 
+// bmb200_scan with BMB200_SCAN_IN: the list -> sorted, unique codes below 2^n_planes in a device buffer of its own, then one
+// scan_in_kernel launch with one result group
+static int scan_in(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* a, bmb200_result** inout)
+{
+    if (!a->n_planes || a->n_planes > 64u) return BMB200_ERR_BADARG;
+    if (a->flags & ~(BMB200_F_COUNT_ONLY | BMB200_F_OPT_COMPRESS | BMB200_F_SIGNED)) return BMB200_ERR_BADARG;
+    if (a->n_values > BMB200_SCAN_IN_MAX_VALUES) return BMB200_ERR_RANGE;
+    if ((uint64_t)a->plane0 + a->n_planes > set->v.n_vec) return BMB200_ERR_RANGE;
+    if (a->universe != 0xffffffffu && a->universe >= set->v.n_vec) return BMB200_ERR_RANGE;
+    const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
+    if (a->nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
+    const uint32_t cols = nb_to - a->nb_from;
+    const bool sgn = (a->flags & BMB200_F_SIGNED) != 0;
+    std::vector<uint64_t> codes;
+    try { codes.reserve(a->n_values); } catch (...) { return BMB200_ERR_BADALLOC; }
+    for (uint32_t k = 0; k < a->n_values; ++k) {
+        const uint64_t v = a->values[k];
+        const uint64_t u = !sgn ? v : (int64_t)v >= 0 ? v << 1 : ((~v) << 1) | 1ull;      // s2u, src/bmbmatrix.h:2536-2569
+        if (a->n_planes < 64u && (u >> a->n_planes)) continue;                              // a bit no plane holds: matches nothing
+        codes.push_back(u);
+    }
+    std::sort(codes.begin(), codes.end());
+    codes.erase(std::unique(codes.begin(), codes.end()), codes.end());
+    CU(cudaSetDevice(ctx->device));
+    const bool store = !(a->flags & BMB200_F_COUNT_ONLY);
+    const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
+
+    bmb200_result* r = *inout;
+    if (r && (r->ctx != ctx || r->n_cols != cols || r->n_groups != 1u || (store && !r->blocks) ||
+              (store && compress && !r->gaps) || r->or_blocks)) {
+        bmb200_result_free(r); r = nullptr; *inout = nullptr;
+    }
+    if (!r) {
+        int rc = result_alloc(ctx, cols, 1u, store, store && compress, false, &r);
+        if (rc) return rc;
+    }
+    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
+    r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
+
+    uint64_t* d_codes = nullptr;
+    int rc = pool_dev(ctx, kDevScanIn, 8 * std::max<size_t>(codes.size(), 1), (void**)&d_codes);
+    if (rc) return bail(rc);
+    // a pageable source: the call returns once the codes are staged, so the vector may go out of scope
+    cudaError_t e = codes.empty() ? cudaSuccess : cudaMemcpyAsync(d_codes, codes.data(), 8 * codes.size(), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
+    const size_t smem = scan_in_smem(a->n_planes);
+    if (e == cudaSuccess && !ctx->scan_in_attr_set) {
+        e = cudaFuncSetAttribute(scan_in_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_in_smem(64));
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(scan_in_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_in_smem(64));
+        ctx->scan_in_attr_set = (e == cudaSuccess);
+    }
+    if (e != cudaSuccess) { ctx->last_err = std::string("scan_in: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
+
+    ScanInParams sp{};
+    sp.out = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
+    sp.out.n_groups = 1u;
+    sp.plane0 = a->plane0; sp.n_planes = a->n_planes; sp.universe = a->universe;
+    sp.n_codes = (uint32_t)codes.size();
+    sp.bucket = sp.n_codes > kInStage ? (sp.n_codes + kInStage - 1u) / kInStage : 0u;     // splitters: one per bucket
+    sp.n_stage = sp.bucket ? (sp.n_codes + sp.bucket - 1u) / sp.bucket : sp.n_codes;
+    sp.codes = d_codes;
+    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
+    if (grid > cols) grid = cols;
+    if (a->n_planes > 32u) scan_in_kernel<true><<<grid, kAggThreads, smem, ctx->stream>>>(sp);
+    else scan_in_kernel<false><<<grid, kAggThreads, smem, ctx->stream>>>(sp);
+    if ((rc = after_launch(ctx))) return bail(rc);
+    *inout = r;
+    if (store && compress) r->gaps_ready = true;
+    return BMB200_OK;
+}
+
 int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* a, bmb200_result** inout)
 {
     if (!ctx || !set || !a || !inout || set->ctx != ctx || !a->values || !a->n_values) return BMB200_ERR_BADARG;
+    if (a->pred == BMB200_SCAN_IN) return scan_in(ctx, set, a, inout);
     if (a->pred < BMB200_SCAN_EQ || a->pred > BMB200_SCAN_RANGE_OPEN || !a->n_planes || a->n_planes > 64u) return BMB200_ERR_BADARG;
     const bool fl = (a->flags & BMB200_F_FLOAT) != 0;
     const bool two = a->pred == BMB200_SCAN_RANGE || a->pred == BMB200_SCAN_RANGE_OPEN;   // two value slots per search

@@ -1,6 +1,8 @@
 // bmb200_scanner.hpp -- reference-side binding: bm::b200::scanner<SV>, the GPU counterpart of
 // bm::sparse_vector_scanner<SV> (src/bmsparsevec_algo.h:1040-1182) for unsigned and signed bm::sparse_vector<> and
 // bm::rsc_sparse_vector<>.
+// The iterator find_eq(first, last, bv_out) (elements equal to any listed value, src/bmsparsevec_algo.h:1398-1423) and
+// count_eq(first, last) are one BMB200_SCAN_IN launch (csrc/scan_in_kernel.cuh) for the whole list.
 //
 // The scanner binds to one sparse vector (like sparse_vector_scanner::bind, :1060): its bit-planes
 // (sparse_vector::get_slice(j), j < effective_slices()) and its searchable universe (the NOT-NULL plane of a nullable
@@ -34,6 +36,7 @@
 #include "bmsparsevec_algo.h"
 #include "bmb200_aggregator.hpp"
 
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <type_traits>
@@ -71,15 +74,17 @@ public:
         }
         n_blocks_ = detail::column_count(std::max<uint64_t>(detail::size_blocks(size_), 1u), "bm::b200::scanner");
         const bvector_type* nn = sv.get_null_bvector();
+        nullable_ = nn != nullptr;
         uint32_t n_vec = n_planes_ + 1;
         if constexpr (SV::is_compressed()) {
             // compressed planes: positions [0, effective_size()); the universe is that range, NN maps it to the logical space
             const size_type eff = sv.effective_size();
             scan_to_ = detail::column_count(std::max<uint64_t>(detail::size_blocks(eff), 1u), "bm::b200::scanner");
             universe_.clear(true); if (eff) universe_.set_range(0, eff - 1); universe_.optimize();
+            if (nn) not_null_ = *nn;
             n_vec = n_planes_ + 2;
         } else {
-            if (nn) universe_ = *nn;                                     // NOT-NULL plane: finalize_search_result(:2426)
+            if (nn) universe_ = not_null_ = *nn;                         // NOT-NULL plane: finalize_search_result(:2426)
             else { universe_.clear(true); if (size_) universe_.set_range(0, size_ - 1); universe_.optimize(); }   // invert_internal(:1686) range
         }
         std::vector<detail::tree_view<bvector_type>> views(n_vec);
@@ -140,6 +145,35 @@ public:
         std::vector<const char*> p(q.size()); for (size_t k = 0; k < q.size(); ++k) p[k] = q[k].c_str();
         counts.assign(q.size(), 0);
         str_run(p.data(), p.size(), 0u, nullptr, counts.data());
+    }
+
+    /// elements equal to any value of [first, last): the iterator find_eq of the reference (src/bmsparsevec_algo.h:1398-1423,
+    /// SQL `IN (...)`) with its effects on bv_out: the result is OR-ed into bv_out, which is not cleared, and when a listed value
+    /// is 0 bv_out is then corrected to the NOT-NULL elements (correct_nulls, :2376) -- bits it held before included.  An empty
+    /// range leaves bv_out untouched.  One BMB200_SCAN_IN launch reads the planes once for the whole list (one launch per
+    /// BMB200_SCAN_IN_MAX_VALUES distinct values).  An RSC vector answers in logical positions, like the OR of find_eq(v).
+    template<class It>
+    void find_eq(It first, It last, bvector_type& bv_out)
+    {
+        bool any_zero = false;
+        std::vector<uint64_t> v = in_slots(first, last, any_zero);
+        if (v.empty()) return;
+        if (size_) {
+            bvector_type r;
+            in_run(v, &r, nullptr);
+            bv_out.bit_or(r);
+        }
+        if (any_zero && nullable_) bv_out.bit_and(not_null_);
+    }
+    /// the number of elements equal to any value of [first, last) (count-only: an RSC vector needs no rank decompression)
+    template<class It>
+    size_type count_eq(It first, It last)
+    {
+        bool any_zero = false;
+        std::vector<uint64_t> v = in_slots(first, last, any_zero);
+        size_type n = 0;
+        if (!v.empty() && size_) in_run(v, nullptr, &n);
+        return n;
     }
 
     /// batched searches: one launch, out[k] replaced by the result of values[k].  For a signed vector every slot holds
@@ -237,12 +271,36 @@ private:
         const uint64_t v[2] = {slot(a), slot(b)};
         run(pred, v, 1, &bv_out, nullptr, is_signed);
     }
+    template<class It>
+    static std::vector<uint64_t> in_slots(It first, It last, bool& any_zero)
+    {
+        static_assert(!SV::is_str(), "a str_sparse_vector is searched with find_eq_str / find_eq_str_batch");
+        std::vector<uint64_t> v;
+        for (; first != last; ++first) { const value_type x = *first; any_zero |= (x == 0); v.push_back(slot(x)); }
+        return v;
+    }
+    /// SCAN_IN over the distinct values of v (sorted and de-duplicated here, so the launches of a long list are disjoint):
+    /// *out replaced by the union, *count = its cardinality
+    void in_run(std::vector<uint64_t>& v, bvector_type* out, size_type* count)
+    {
+        std::sort(v.begin(), v.end());
+        v.erase(std::unique(v.begin(), v.end()), v.end());
+        if (count) *count = 0;
+        for (size_t k0 = 0; k0 < v.size(); k0 += BMB200_SCAN_IN_MAX_VALUES) {
+            const uint32_t nv = (uint32_t)std::min<size_t>(v.size() - k0, BMB200_SCAN_IN_MAX_VALUES);
+            bvector_type part; size_type n = 0;
+            run(BMB200_SCAN_IN, v.data() + k0, nv, out ? &part : nullptr, &n, is_signed);
+            if (count) *count += n;
+            if (out) { if (k0) out->bit_or(part); else out->swap(part); }
+        }
+    }
     void run(int pred, const uint64_t* values, uint32_t nv, bvector_type* out, size_type* counts, bool sgn)
     {
         static_assert(!SV::is_str(), "a str_sparse_vector is searched with find_eq_str / find_eq_str_prefix");
         if (!nv) return;
         const uint32_t flags = (out ? BMB200_F_OPT_COMPRESS : BMB200_F_COUNT_ONLY) | (sgn ? BMB200_F_SIGNED : 0u);
         bmb200_scan_args a{0u, n_planes_, n_planes_, pred, flags, values, nv, 0u, scan_to_};
+        if (pred == BMB200_SCAN_IN) nv = 1u;                       // one list, one result group
         bmb200_result* res = nullptr;
         int rc = bmb200_scan(ctx_.get(), set_, &a, &res);
         if constexpr (SV::is_compressed()) {
@@ -274,6 +332,8 @@ private:
     bmb200_rs* rs_ = nullptr;          // RSC: rs index of NN
     const SV* str_sv_ = nullptr;       // string vector: its remap tables stay on the host (to_codes)
     bvector_type universe_;
+    bvector_type not_null_;            // nullable vectors: the NOT-NULL vector (logical positions), for correct_nulls
+    bool nullable_ = false;
     size_type size_ = 0;
     unsigned n_planes_ = 0;
     uint32_t n_blocks_ = 0;

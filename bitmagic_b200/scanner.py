@@ -24,6 +24,11 @@ Float vectors (``bm::sparse_vector_float<sparse_vector<unsigned>>``, ``SparseVec
 searches (``find_gt_float`` & co.) run with ``F_FLOAT`` and float32 values.  They compare in the IEEE sign-magnitude total
 order of the bits (-0 < +0, NaNs beyond the infinities), as the reference's float searches do; there is no float ``find_eq``.
 
+``find_eq_any(values)`` / ``count_eq_any(values)`` are the reference's iterator ``find_eq(sv, start, end, bv_out)``
+(src/bmsparsevec_algo.h:1398-1423, SQL ``IN (...)``) for plain, nullable, RSC and signed vectors: one ``SCAN_IN`` launch reads
+the planes once for the whole list (csrc/scan_in_kernel.cuh).  They return the set of matching elements; an RSC vector answers
+in logical positions.
+
 String vectors (``bm::str_sparse_vector<char, ...>``, ``StrSparseVector``) keep bit b of byte k of every element in plane 8k+b;
 ``find_eq_str`` / ``find_eq_str_prefix`` / ``count_eq_str`` run as ``bmb200_scan_str`` (csrc/str_scan_kernel.cuh).  The numeric
 searches raise on a string vector.
@@ -33,8 +38,8 @@ from __future__ import annotations
 import numpy as np
 
 from . import capi
-from .capi import (F_COUNT_ONLY, F_FLOAT, F_OPT_COMPRESS, F_SIGNED, F_STR_PREFIX, SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_LE, SCAN_LT,
-                   SCAN_RANGE, SCAN_RANGE_OPEN)
+from .capi import (F_COUNT_ONLY, F_FLOAT, F_OPT_COMPRESS, F_SIGNED, F_STR_PREFIX, SCAN_EQ, SCAN_GE, SCAN_GT, SCAN_IN, SCAN_LE,
+                   SCAN_LT, SCAN_RANGE, SCAN_RANGE_OPEN)
 from .hostfmt import BLOCK_BITS, BVector, PackedSet, bits_to_words, result_to_bvector
 
 
@@ -243,6 +248,20 @@ class SparseVectorScanner:
         res = capi.scan(self.ctx, self._dset, pred, vals, 0, self.sv.effective_slices(), self._universe, flags, 0, self._scan_to)
         return self._results(res, vals.shape[0], count_only, single)
 
+    def _run_in(self, values, count_only=False):
+        """elements equal to any of `values` (one SCAN_IN launch); the list is de-duplicated here, and may then hold at most
+        capi.SCAN_IN_MAX_VALUES values"""
+        if self._str or self._float:
+            raise TypeError("find_eq_any / count_eq_any search integer vectors (the reference has no float or string list form)")
+        vals = np.unique(np.atleast_1d(np.asarray(values, np.int64 if self.sv.signed else np.uint64)))
+        if vals.ndim != 1:
+            raise ValueError("find_eq_any takes a 1-D list of values")
+        if not vals.size:
+            return 0 if count_only else BVector(self._n_blocks)
+        flags = (F_COUNT_ONLY if count_only else F_OPT_COMPRESS) | (F_SIGNED if self.sv.signed else 0)
+        res = capi.scan(self.ctx, self._dset, SCAN_IN, vals, 0, self.sv.effective_slices(), self._universe, flags, 0, self._scan_to)
+        return self._results(res, 1, count_only, True)
+
     def _run_str(self, strs, prefix, count_only=False):
         if not self._str:
             raise TypeError("string searches need a StrSparseVector")
@@ -290,6 +309,9 @@ class SparseVectorScanner:
     def count_gt(self, value):   return self._run(SCAN_GT, value, True)
     def count_range(self, lo, hi=None):
         return self._run(SCAN_RANGE, [lo, hi] if hi is not None else lo, True)
+    # set membership, SQL `IN (...)`: the elements equal to any listed value, NULLs excluded (a fresh result, not OR-ed into one)
+    def find_eq_any(self, values):   return self._run_in(values)
+    def count_eq_any(self, values):  return self._run_in(values, True)
     # float vectors: float32 values (one, or a list = one launch); ranges as (from, to) or a list of such rows
     def find_gt_float(self, value):  return self._run(SCAN_GT, value, fl=True)
     def find_ge_float(self, value):  return self._run(SCAN_GE, value, fl=True)

@@ -23,6 +23,7 @@
  *   bmb200_set_upload_blobs       <- bm::deserialize / deserializer<BV>::deserialize  src/bmserial.h:4152,5578-6090
  *   bmb200_scan                   <- sparse_vector_scanner::find_eq/find_gt/find_ge/find_lt/find_le/find_range
  *                                                                   src/bmsparsevec_algo.h:1083-1182,2593-2632,4360-4395
+ *   bmb200_scan  BMB200_SCAN_IN   <- sparse_vector_scanner::find_eq(sv, start, end, bv_out)  src/bmsparsevec_algo.h:1398-1423
  *   bmb200_scan  BMB200_F_FLOAT   <- sparse_vector_scanner::find_gt_float/find_ge_float/find_lt_float/find_le_float/
  *                                    find_range_float/find_range_float_unbounded over sparse_vector_float
  *                                                                   src/bmsparsevec_algo.h:1299-1352,3692-4009
@@ -377,6 +378,17 @@ int bmb200_result_free(bmb200_result* res);
 #define BMB200_SCAN_LE     4   /* find_le    :1163                                                             */
 #define BMB200_SCAN_RANGE  5   /* find_range :1174  values[2k] <= element <= values[2k+1] (reversed bounds are swapped, :2871) */
 #define BMB200_SCAN_RANGE_OPEN 6 /* find_range_float_unbounded :3841  values[2k] < element < values[2k+1]; BMB200_F_FLOAT only */
+/* Set membership (sparse_vector_scanner::find_eq(sv, start, end, bv_out), src/bmsparsevec_algo.h:1398-1423; SQL `IN (...)`):
+ * values[0..n_values) is ONE list -- uint64_t codes, or int64_t in two's complement with BMB200_F_SIGNED -- in any order,
+ * duplicates allowed.  The result has ONE group of n_cols columns: U & {i : code(i) in codes(list)}, where code is the stored
+ * code (s2u(x) with BMB200_F_SIGNED) and U the universe; value 0 matches the zero elements inside U only (find_zero), codes with
+ * a bit at or above n_planes match nothing.  The library applies s2u, sorts, de-duplicates and drops such codes on the host; one
+ * launch reads every plane block once, whatever the list's length (csrc/scan_in_kernel.cuh).  The count is
+ * bmb200_result_group_totals(res, &t, 1).  flags: BMB200_F_COUNT_ONLY / BMB200_F_OPT_NONE / BMB200_F_OPT_COMPRESS, | BMB200_F_SIGNED.
+ * BMB200_ERR_BADARG for BMB200_F_FLOAT (the reference has no float find_eq), any other flag and n_values == 0;
+ * BMB200_ERR_RANGE for n_values > BMB200_SCAN_IN_MAX_VALUES. */
+#define BMB200_SCAN_IN     7
+#define BMB200_SCAN_IN_MAX_VALUES (1u << 20)
 typedef struct bmb200_scan_args {
     uint32_t        plane0;     /* first plane vector inside the set                                          */
     uint32_t        n_planes;   /* 1..64 (sparse_vector::effective_slices()); BMB200_F_FLOAT: 1..32           */
