@@ -46,7 +46,7 @@ SYMBOLS = [
     "bmb200_result_fetch_view_async", "bmb200_result_fetch_wait", "bmb200_exchange_mode",
     "bmb200_result_fetch_column", "bmb200_set_run_lists", "bmb200_set_bit_run_lists",
     "bmb200_rank_decompress", "bmb200_rank_compress", "bmb200_scan_str", "bmb200_set_packed_singles",
-    "bmb200_set_run_list_unions", "bmb200_set_coverage",
+    "bmb200_set_run_list_unions", "bmb200_set_coverage", "bmb200_sv_mismatch", "bmb200_sv_first_mismatch",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
@@ -106,6 +106,16 @@ class ScanStrArgsC(C.Structure):
         ("nb_from", C.c_uint32), ("nb_to", C.c_uint32),
     ]
 
+
+class MismatchArgsC(C.Structure):
+    _fields_ = [
+        ("plane0_a", C.c_uint32), ("n_planes_a", C.c_uint32), ("plane0_b", C.c_uint32), ("n_planes_b", C.c_uint32),
+        ("not_null_a", C.c_uint32), ("not_null_b", C.c_uint32), ("size_a", C.c_uint64), ("size_b", C.c_uint64),
+        ("null_proc", C.c_uint32), ("flags", C.c_uint32), ("nb_from", C.c_uint32), ("nb_to", C.c_uint32),
+    ]
+
+
+MM_NO_NULL, MM_USE_NULL = 0, 1   # bm::no_null / bm::use_null of the mismatch functions
 
 SCAN_EQ, SCAN_GT, SCAN_GE, SCAN_LT, SCAN_LE, SCAN_RANGE = range(6)
 SCAN_RANGE_OPEN = 6           # lo < element < hi (find_range_float_unbounded); F_FLOAT only
@@ -632,6 +642,32 @@ def scan_str(ctx: Context, dset: DeviceSet, strs, plane0: int, n_planes: int, un
     ctx.check(lib().bmb200_scan_str(ctx._h, dset._h, C.byref(args), C.byref(res._h)), "scan_str")
     res.n_cols = ((nb_to if nb_to else dset.n_blocks) - nb_from) * int(nv)
     return res
+
+
+def mismatch_args(plane0_a: int, n_planes_a: int, plane0_b: int, n_planes_b: int, not_null_a: int = NO_UNIVERSE,
+                  not_null_b: int = NO_UNIVERSE, size_a: int = 0, size_b: int = 0, null_proc: int = MM_USE_NULL, flags: int = 0,
+                  nb_from: int = 0, nb_to: int = 0) -> MismatchArgsC:
+    """bmb200_mismatch_args: sv1's planes are set vectors plane0_a.., sv2's plane0_b..; not_null_* = NO_UNIVERSE for a
+    non-nullable vector"""
+    return MismatchArgsC(int(plane0_a), int(n_planes_a), int(plane0_b), int(n_planes_b), int(not_null_a), int(not_null_b),
+                         int(size_a), int(size_b), int(null_proc), int(flags), int(nb_from), int(nb_to))
+
+
+def sv_mismatch(ctx: Context, dset: DeviceSet, args: MismatchArgsC, result: DeviceResult | None = None) -> DeviceResult:
+    """bmb200_sv_mismatch (sparse_vector_find_mismatch): the positions where the two vectors differ, one group of n_cols
+    columns (its count: group_totals(1))"""
+    res = result if result is not None else DeviceResult(ctx)
+    ctx.check(lib().bmb200_sv_mismatch(ctx._h, dset._h, C.byref(args), C.byref(res._h)), "sv_mismatch")
+    res.n_cols = (args.nb_to if args.nb_to else dset.n_blocks) - args.nb_from
+    return res
+
+
+def sv_first_mismatch(ctx: Context, dset: DeviceSet, args: MismatchArgsC) -> int | None:
+    """bmb200_sv_first_mismatch (sparse_vector_find_first_mismatch): the lowest position where the two vectors differ, or
+    None"""
+    pos, found = C.c_uint64(0), C.c_int(0)
+    ctx.check(lib().bmb200_sv_first_mismatch(ctx._h, dset._h, C.byref(args), C.byref(pos), C.byref(found)), "sv_first_mismatch")
+    return int(pos.value) if found.value else None
 
 
 def _sized(res: DeviceResult) -> DeviceResult:

@@ -13,6 +13,7 @@
 #include "runlist_kernel.cuh"
 #include "scan_kernel.cuh"
 #include "scan_in_kernel.cuh"
+#include "mismatch_kernel.cuh"
 #include "str_scan_kernel.cuh"
 #include "rank_kernel.cuh"
 #include "shift_kernel.cuh"
@@ -52,6 +53,7 @@ enum DevSlot {
     kDevBlobRecs, kDevBlobERecs,      //   decode records: explicit-length tokens, entropy-coded tokens
     kDevBlobDur,                      //   pass 2: clocks per work item (BMB200_TRACE)
     kDevScanIn,                       // bmb200_scan BMB200_SCAN_IN: the sorted, unique code list
+    kDevFirstMismatch,                // bmb200_sv_first_mismatch: the lowest mismatch position (one u64)
     kDevSlots
 };
 enum HostSlot {
@@ -1765,6 +1767,94 @@ static int scan_in(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_arg
     if ((rc = after_launch(ctx))) return bail(rc);
     *inout = r;
     if (store && compress) r->gaps_ready = true;
+    return BMB200_OK;
+}
+
+// bmb200_sv_mismatch / bmb200_sv_first_mismatch: argument checks shared by both forms; *cols = columns of the launch
+static int mismatch_check(const bmb200_set* set, const bmb200_mismatch_args* a, uint32_t* cols)
+{
+    const uint32_t M = set->v.n_vec, kNone = 0xffffffffu;
+    if (a->null_proc > BMB200_MM_USE_NULL || (a->flags & ~(BMB200_F_COUNT_ONLY | BMB200_F_OPT_COMPRESS))) return BMB200_ERR_BADARG;
+    if (a->n_planes_a > 64u || a->n_planes_b > 64u) return BMB200_ERR_BADARG;
+    if ((uint64_t)a->plane0_a + a->n_planes_a > M || (uint64_t)a->plane0_b + a->n_planes_b > M) return BMB200_ERR_BADARG;
+    if ((a->not_null_a != kNone && a->not_null_a >= M) || (a->not_null_b != kNone && a->not_null_b >= M)) return BMB200_ERR_BADARG;
+    const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
+    if (a->nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
+    *cols = nb_to - a->nb_from;
+    return BMB200_OK;
+}
+
+static MismatchParams mismatch_params(const bmb200_mismatch_args* a)
+{
+    MismatchParams mp{};
+    mp.plane0_a = a->plane0_a; mp.n_planes_a = a->n_planes_a; mp.plane0_b = a->plane0_b; mp.n_planes_b = a->n_planes_b;
+    mp.not_null_a = a->not_null_a; mp.not_null_b = a->not_null_b;
+    mp.size_a = a->size_a; mp.size_b = a->size_b;
+    mp.use_null = a->null_proc == BMB200_MM_USE_NULL ? 1u : 0u;
+    return mp;
+}
+
+int bmb200_sv_mismatch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_mismatch_args* a, bmb200_result** inout)
+{
+    if (!ctx || !set || !a || !inout || set->ctx != ctx) return BMB200_ERR_BADARG;
+    uint32_t cols = 0;
+    int rc = mismatch_check(set, a, &cols);
+    if (rc) return rc;
+    CU(cudaSetDevice(ctx->device));
+    const bool store = !(a->flags & BMB200_F_COUNT_ONLY);
+    const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
+
+    bmb200_result* r = *inout;
+    if (r && (r->ctx != ctx || r->n_cols != cols || r->n_groups != 1u || (store && !r->blocks) ||
+              (store && compress && !r->gaps) || r->or_blocks)) {
+        bmb200_result_free(r); r = nullptr; *inout = nullptr;
+    }
+    if (!r) {
+        if ((rc = result_alloc(ctx, cols, 1u, store, store && compress, false, &r))) return rc;
+    }
+    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
+    r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
+    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
+    if (e != cudaSuccess) { ctx->last_err = std::string("sv_mismatch: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
+
+    MismatchParams mp = mismatch_params(a);
+    mp.out = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
+    mp.out.n_groups = 1u;
+    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
+    if (grid > cols) grid = cols;
+    mismatch_kernel<false><<<grid, kAggThreads, 0, ctx->stream>>>(mp);
+    if ((rc = after_launch(ctx))) return bail(rc);
+    *inout = r;
+    if (store && compress) r->gaps_ready = true;
+    return BMB200_OK;
+}
+
+int bmb200_sv_first_mismatch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_mismatch_args* a, uint64_t* pos, int* found)
+{
+    if (!ctx || !set || !a || !pos || !found || set->ctx != ctx) return BMB200_ERR_BADARG;
+    uint32_t cols = 0;
+    int rc = mismatch_check(set, a, &cols);
+    if (rc) return rc;
+    CU(cudaSetDevice(ctx->device));
+    unsigned long long* d_first = nullptr;
+    if ((rc = pool_dev(ctx, kDevFirstMismatch, 8, (void**)&d_first))) return rc;
+    CU(cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream));
+    CU(cudaMemsetAsync(d_first, 0xff, 8, ctx->stream));
+
+    MismatchParams mp = mismatch_params(a);
+    mp.out.set = set->v; mp.out.nb_from = a->nb_from; mp.out.n_cols = cols; mp.out.n_groups = 1u;
+    mp.out.work_counter = ctx->d_work;
+    mp.first = d_first;
+    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
+    if (grid > cols) grid = cols;
+    mismatch_kernel<true><<<grid, kAggThreads, 0, ctx->stream>>>(mp);
+    if ((rc = after_launch(ctx))) return rc;
+    unsigned long long h = ~0ull;
+    CU(cudaMemcpyAsync(&h, d_first, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    *pos = (uint64_t)h;
+    *found = h != ~0ull;
     return BMB200_OK;
 }
 

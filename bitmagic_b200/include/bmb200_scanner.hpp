@@ -29,6 +29,8 @@
 // exponents_.get_slice(0..7) as the planes of one BMB200_F_FLOAT scan and offers the reference's find_gt_float / find_ge_float /
 // find_lt_float / find_le_float / find_range_float / find_range_float_unbounded plus batched and count-only forms.
 // bm::b200::rank_compressor<BV> is the device counterpart of bm::rank_compressor<BV> (src/bmalgo.h:451-644).
+// bm::b200::sparse_vector_find_mismatch / sparse_vector_find_first_mismatch compare two plain integer sparse vectors
+// (src/bmsparsevec_algo.h:479,657) in one bmb200_sv_mismatch / bmb200_sv_first_mismatch launch (csrc/mismatch_kernel.cuh).
 #ifndef BMB200_SCANNER_HPP_INCLUDED
 #define BMB200_SCANNER_HPP_INCLUDED
 
@@ -518,6 +520,103 @@ private:
     }
     context& ctx_;
 };
+
+// ---- sparse-vector mismatch: sparse_vector_find_mismatch / sparse_vector_find_first_mismatch, src/bmsparsevec_algo.h:479,657 ----
+namespace detail {
+
+/// plain integer sparse vectors only: rsc_sparse_vector (the reference asserts in the vector form and compares compressed
+/// positions in the first form), str_sparse_vector and sparse_vector_float are out of scope
+template<class SV> struct mismatch_vector : std::false_type {};
+template<class T, class BV> struct mismatch_vector<bm::sparse_vector<T, BV>>
+    : std::integral_constant<bool, std::is_integral<T>::value && (sizeof(T) == 4 || sizeof(T) == 8)> {};
+
+/// both vectors of a comparison uploaded into one set: the trimmed planes of sv1, then of sv2, then the NOT-NULL vectors of
+/// the nullable ones, with columns covering max(sv1.size(), sv2.size()) (uploaded per call, like rank_compressor)
+template<class SV>
+struct mismatch_set
+{
+    typedef typename SV::bvector_type bvector_type;
+    bmb200_set* set = nullptr;
+    bmb200_mismatch_args args{};
+    uint32_t n_blocks = 0;
+
+    mismatch_set(context& ctx, const SV& sv1, const SV& sv2, bm::null_support null_proc, const char* what)
+    {
+        static_assert(mismatch_vector<SV>::value,
+                      "bm::b200 mismatch compares bm::sparse_vector<unsigned / unsigned long long / int32_t / int64_t> only");
+        std::vector<const bvector_type*> vecs;
+        const unsigned na = planes(sv1, vecs), nb = planes(sv2, vecs);
+        const bvector_type* nn1 = sv1.get_null_bvector();
+        const bvector_type* nn2 = sv2.get_null_bvector();
+        args.plane0_a = 0u; args.n_planes_a = na; args.plane0_b = na; args.n_planes_b = nb;
+        args.not_null_a = nn1 ? (uint32_t)vecs.size() : 0xffffffffu; if (nn1) vecs.push_back(nn1);
+        args.not_null_b = nn2 ? (uint32_t)vecs.size() : 0xffffffffu; if (nn2) vecs.push_back(nn2);
+        args.size_a = uint64_t(sv1.size()); args.size_b = uint64_t(sv2.size());
+        args.null_proc = null_proc == bm::use_null ? BMB200_MM_USE_NULL : BMB200_MM_NO_NULL;
+        n_blocks = column_count(std::max<uint64_t>(size_blocks(std::max(args.size_a, args.size_b)), 1u), what);
+        const uint32_t n_vec = std::max<uint32_t>((uint32_t)vecs.size(), 1u);
+        std::vector<tree_view<bvector_type>> views(n_vec);
+        std::vector<bmb200_vec_blocks> vb(n_vec);
+        bvector_type empty;
+        for (uint32_t j = 0; j < n_vec; ++j) {
+            views[j].build(j < vecs.size() ? *vecs[j] : empty, n_blocks);
+            vb[j].n_blocks = n_blocks; vb[j].kind = views[j].kind.data(); vb[j].ptr = views[j].ptr.data();
+        }
+        check(bmb200_set_upload_vectors(ctx.get(), n_vec, n_blocks, vb.data(), &set), "bmb200_set_upload_vectors");
+    }
+    ~mismatch_set() { if (set) bmb200_set_free(set); }
+    mismatch_set(const mismatch_set&) = delete; mismatch_set& operator=(const mismatch_set&) = delete;
+
+    /// the value planes j < effective_slices() (an absent one as an empty vector), trailing absent ones trimmed -> their count
+    static unsigned planes(const SV& sv, std::vector<const bvector_type*>& vecs)
+    {
+        static const bvector_type empty;
+        unsigned n = sv.effective_slices();
+        auto at = [&](unsigned j) { const bvector_type* bv = sv.get_slice(j); return bv == sv.get_null_bvector() ? nullptr : bv; };
+        while (n && !at(n - 1)) --n;
+        for (unsigned j = 0; j < n; ++j) { const bvector_type* bv = at(j); vecs.push_back(bv ? bv : &empty); }
+        return n;
+    }
+};
+
+} // namespace detail
+
+/// bm::sparse_vector_find_mismatch (src/bmsparsevec_algo.h:657) on the device: bv = the positions where sv1 and sv2 differ
+/// (values, sizes, and under bm::use_null the NULLs; bm::no_null leaves positions NULL in both vectors out).  One
+/// bmb200_sv_mismatch launch over both vectors' planes.  With bm::use_null and two non-nullable vectors the reference reports
+/// every position [0, bm::id_max) (it inverts an empty vector); here no NULL term is added (DESIGN.md 3.5f).
+template<class SV>
+void sparse_vector_find_mismatch(context& ctx, typename SV::bvector_type& bv, const SV& sv1, const SV& sv2, bm::null_support null_proc)
+{
+    detail::mismatch_set<SV> ms(ctx, sv1, sv2, null_proc, "bm::b200::sparse_vector_find_mismatch");
+    ms.args.flags = BMB200_F_OPT_COMPRESS;
+    bmb200_result* res = nullptr;
+    int rc = bmb200_sv_mismatch(ctx.get(), ms.set, &ms.args, &res);
+    std::vector<uint8_t> kind(ms.n_blocks); std::vector<uint64_t> off(ms.n_blocks);
+    std::vector<uint32_t> bits; std::vector<uint16_t> gaps;
+    uint64_t nb = 0, ng = 0;
+    if (!rc) rc = bmb200_result_sizes(res, &nb, &ng);
+    if (!rc) { bits.resize(nb * BMB200_BLOCK_WORDS); gaps.resize(ng); rc = bmb200_result_fetch(res, kind.data(), off.data(), bits.data(), gaps.data()); }
+    if (res) bmb200_result_free(res);
+    check(rc, "bmb200_sv_mismatch");
+    bv.clear(true);                                                  // replaced, as the reference's bv.clear()
+    detail::store_result(bv, bv.size(), ms.n_blocks, kind.data(), off.data(), bits.data(), gaps.data());
+}
+
+/// bm::sparse_vector_find_first_mismatch (src/bmsparsevec_algo.h:479) on the device: the lowest position where sv1 and sv2
+/// differ -> true and midx, or false and midx = bm::id_max.  One bmb200_sv_first_mismatch launch; 8 bytes come back.  The
+/// reference compares GAP x GAP blocks by run ends only and can miss or postpone a difference there; this returns the true
+/// lowest position (DESIGN.md 3.5f).
+template<class SV>
+bool sparse_vector_find_first_mismatch(context& ctx, const SV& sv1, const SV& sv2, typename SV::size_type& midx,
+                                       bm::null_support null_proc = bm::use_null)
+{
+    detail::mismatch_set<SV> ms(ctx, sv1, sv2, null_proc, "bm::b200::sparse_vector_find_first_mismatch");
+    uint64_t pos = 0; int found = 0;
+    check(bmb200_sv_first_mismatch(ctx.get(), ms.set, &ms.args, &pos, &found), "bmb200_sv_first_mismatch");
+    midx = found ? (typename SV::size_type)pos : (typename SV::size_type)bm::id_max;
+    return found != 0;
+}
 
 }} // namespace bm::b200
 

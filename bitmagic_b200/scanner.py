@@ -29,6 +29,10 @@ order of the bits (-0 < +0, NaNs beyond the infinities), as the reference's floa
 the planes once for the whole list (csrc/scan_in_kernel.cuh).  They return the set of matching elements; an RSC vector answers
 in logical positions.
 
+``find_mismatch(sv1, sv2)`` / ``find_first_mismatch(sv1, sv2)`` are the reference's ``sparse_vector_find_mismatch`` /
+``sparse_vector_find_first_mismatch`` (src/bmsparsevec_algo.h:657,479) for two plain ``SparseVector``s: both vectors'
+planes and NOT-NULL vectors go into one set and one launch reads every plane block once (csrc/mismatch_kernel.cuh).
+
 String vectors (``bm::str_sparse_vector<char, ...>``, ``StrSparseVector``) keep bit b of byte k of every element in plane 8k+b;
 ``find_eq_str`` / ``find_eq_str_prefix`` / ``count_eq_str`` run as ``bmb200_scan_str`` (csrc/str_scan_kernel.cuh).  The numeric
 searches raise on a string vector.
@@ -333,3 +337,50 @@ class SparseVectorScanner:
     def find_eq_str(self, s):         return self._run_str(s, False)
     def find_eq_str_prefix(self, s):  return self._run_str(s, True)
     def count_eq_str(self, s):        return self._run_str(s, False, True)
+
+
+def _mismatch_set(sv1: SparseVector, sv2: SparseVector, use_null: bool, ctx):
+    """both vectors' planes, then their NOT-NULL vectors, in one uploaded set with columns covering max(size) -> dset, args"""
+    for sv in (sv1, sv2):
+        if type(sv) is not SparseVector:
+            raise TypeError("find_mismatch / find_first_mismatch compare two plain SparseVector (not RSC, float or string)")
+    vecs = list(sv1.planes) + list(sv2.planes)
+    nn = []
+    for sv in (sv1, sv2):
+        nn.append(len(vecs) if sv.not_null is not None else capi.NO_UNIVERSE)
+        if sv.not_null is not None:
+            vecs.append(sv.not_null)
+    nb = max([max(1, (max(sv1.size, sv2.size) + BLOCK_BITS - 1) // BLOCK_BITS)] + [v.n_blocks for v in vecs])
+    dset = capi.DeviceSet.upload(ctx, PackedSet.pack(vecs, nb))
+    args = capi.mismatch_args(0, len(sv1.planes), len(sv1.planes), len(sv2.planes), nn[0], nn[1], sv1.size, sv2.size,
+                              capi.MM_USE_NULL if use_null else capi.MM_NO_NULL, F_OPT_COMPRESS)
+    return dset, args
+
+
+def find_mismatch(sv1: SparseVector, sv2: SparseVector, use_null: bool = True, ctx: capi.Context | None = None) -> BVector:
+    """sparse_vector_find_mismatch(bv, sv1, sv2, use_null ? bm::use_null : bm::no_null): the positions where the vectors'
+    values or sizes differ, and with use_null where exactly one of them is NULL (without it, positions NULL in both vectors
+    are left out).  With use_null and two non-nullable vectors the reference reports every position up to bm::id_max; this
+    adds no NULL term there (DESIGN.md 3.5f)."""
+    ctx = ctx or capi.default_context()
+    dset, args = _mismatch_set(sv1, sv2, use_null, ctx)
+    res = None
+    try:
+        res = capi.sv_mismatch(ctx, dset, args)
+        return result_to_bvector(*res.fetch())
+    finally:
+        if res is not None:
+            res.free()
+        dset.free()
+
+
+def find_first_mismatch(sv1: SparseVector, sv2: SparseVector, use_null: bool = True, ctx: capi.Context | None = None) -> int | None:
+    """sparse_vector_find_first_mismatch(sv1, sv2, midx, ...): the lowest position where the vectors differ, None when they
+    do not (the reference then returns false and bm::id_max).  The reference can miss or postpone a difference inside two GAP
+    blocks; this returns the true lowest position (DESIGN.md 3.5f)."""
+    ctx = ctx or capi.default_context()
+    dset, args = _mismatch_set(sv1, sv2, use_null, ctx)
+    try:
+        return capi.sv_first_mismatch(ctx, dset, args)
+    finally:
+        dset.free()

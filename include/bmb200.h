@@ -29,6 +29,8 @@
  *                                                                   src/bmsparsevec_algo.h:1299-1352,3692-4009
  *   bmb200_scan_str               <- sparse_vector_scanner::find_eq_str / find_eq_str_prefix / find_eq_str(TPipe&) over
  *                                    str_sparse_vector            src/bmsparsevec_algo.h:2546-2588,3263-3436,4579-4651
+ *   bmb200_sv_mismatch            <- sparse_vector_find_mismatch   src/bmsparsevec_algo.h:657
+ *   bmb200_sv_first_mismatch      <- sparse_vector_find_first_mismatch  src/bmsparsevec_algo.h:479
  *   bmb200_rs_build               <- bvector::build_rs_index       src/bm.h:2531-2660, rs_index src/bmrs.h:688-715
  *   bmb200_rank_batch             <- bvector::count_to             src/bm.h:3120-3167
  *   bmb200_select_batch           <- bvector::select               src/bm.h:5350-5385
@@ -429,6 +431,47 @@ typedef struct bmb200_scan_str_args {
 } bmb200_scan_str_args;
 /* BMB200_ERR_BADARG also for n_planes > 2048 and for a slot without a NUL */
 int bmb200_scan_str(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_str_args* args, bmb200_result** inout);
+
+/* ---------------- sparse-vector mismatch (where two vectors differ) ---------------- */
+/* sparse_vector_find_mismatch(bv, sv1, sv2, null_proc) (src/bmsparsevec_algo.h:657) and
+ * sparse_vector_find_first_mismatch(sv1, sv2, midx, null_proc) (:479) over two plain sparse vectors A and B stored in ONE
+ * set: A_j = set vector plane0_a + j (j < n_planes_a), B_j = plane0_b + j (j < n_planes_b), an absent plane is empty; NA / NB
+ * are the NOT-NULL vectors of nullable vectors (0xffffffff = not nullable), sa / sb the vectors' size().  [x, y) is the bit
+ * range x..y-1, clipped to the columns of the set.  The planes run over j < max(n_planes_a, n_planes_b).
+ *   bmb200_sv_mismatch (vector form):
+ *     D = OR_j (A_j ^ B_j) | [min(sa, sb), max(sa, sb))
+ *     BMB200_MM_USE_NULL: both nullable D |= NA ^ NB; only A D |= [0, sa) & ~NA; only B D |= [0, sb) & ~NB; neither: nothing
+ *     BMB200_MM_NO_NULL:  both nullable D &= NA | NB; only one D &= its NOT-NULL vector; neither: nothing
+ *   The result is ONE group of n_cols columns (count: bmb200_result_group_totals(res, &t, 1)); results are recycled as usual.
+ *   flags: BMB200_F_OPT_NONE / BMB200_F_OPT_COMPRESS / BMB200_F_COUNT_ONLY.
+ *   The reference's use_null branch with two non-nullable vectors inverts an empty bvector and so reports [0, bm::id_max);
+ *   here it adds nothing (DESIGN.md 3.5f).
+ *   bmb200_sv_first_mismatch: *pos = the lowest set bit of
+ *     F = OR_j (A_j ^ B_j)
+ *     BMB200_MM_USE_NULL: both nullable F |= NA ^ NB; only A F |= NA ^ [0, sb); only B F |= NB ^ [0, sa)
+ *   (no size range, no NOT-NULL mask; BMB200_MM_NO_NULL compares the planes only) inside columns [nb_from, nb_to);
+ *   *found = 1, or *found = 0 and *pos = UINT64_MAX (bm::id_max) when F is empty there.  flags are checked as for
+ *   bmb200_sv_mismatch and otherwise ignored (nothing is stored).  The reference
+ *   compares GAP x GAP blocks by run ends only and can miss or postpone a first difference there; this returns the true
+ *   lowest bit (DESIGN.md 3.5f).
+ * One launch reads every stored plane block of both vectors once per column (csrc/mismatch_kernel.cuh); both vectors may sit
+ * anywhere in the set, so many resident versions of a column can be compared pairwise without uploading again.
+ * BMB200_ERR_BADARG for any other null_proc or flag, n_planes_a or n_planes_b above 64, planes or NOT-NULL ids outside the
+ * set; column ranges as bmb200_scan (BMB200_ERR_RANGE). */
+#define BMB200_MM_NO_NULL  0   /* bm::no_null  */
+#define BMB200_MM_USE_NULL 1   /* bm::use_null */
+typedef struct bmb200_mismatch_args {
+    uint32_t plane0_a, n_planes_a;   /* planes of sv1: set vectors plane0_a .. plane0_a + n_planes_a - 1 (n_planes_a 0..64) */
+    uint32_t plane0_b, n_planes_b;   /* planes of sv2 (0..64)                                                               */
+    uint32_t not_null_a, not_null_b; /* NOT-NULL vectors; 0xffffffff = the vector is not nullable                           */
+    uint64_t size_a, size_b;         /* sv1.size(), sv2.size()                                                              */
+    uint32_t null_proc;              /* BMB200_MM_NO_NULL / BMB200_MM_USE_NULL                                              */
+    uint32_t flags;                  /* bmb200_sv_mismatch: BMB200_F_OPT_NONE / BMB200_F_OPT_COMPRESS / BMB200_F_COUNT_ONLY */
+    uint32_t nb_from;
+    uint32_t nb_to;                  /* 0 == n_blocks */
+} bmb200_mismatch_args;
+int bmb200_sv_mismatch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_mismatch_args* args, bmb200_result** inout);
+int bmb200_sv_first_mismatch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_mismatch_args* args, uint64_t* pos, int* found);
 
 /* end-to-end convenience: HOST packed set in, HOST metadata out, in one call: H2D of the whole set (every call), kernel,
  * D2H of the per-column metadata requested in meta_out (kind / popcnt / digest / nruns) and of the cardinality.  The result
