@@ -207,8 +207,7 @@ __global__ void __launch_bounds__(256) rs_block_kernel(const SetView set, uint32
         uint32_t tot = 0, le0 = 0, le1 = 0, a0 = 0, a1 = 0;
         uint32_t* fout = fine + (size_t)nb * kRsWin;
         if (kd == BMB200_BLK_GAP) {
-            const uint16_t* unit = set.gap_pool + (set.gap_base[nb] + (rel & BMB200_DESC_REL_MASK)) * (size_t)kGapUnit;
-            const uint32_t pad = rel >> 29;
+            const auto [unit, pad] = gap_block_addr(set.gap_pool + set.gap_base[nb] * (size_t)kGapUnit, d);
             const uint32_t hdr = unit[pad], len = hdr >> 3, first = hdr & 1u;
             __syncwarp();
             {
@@ -428,7 +427,7 @@ __global__ void __launch_bounds__(256) rs_rank_kernel(const RsView rs, const uin
                     }
                 }
             } else {
-                const uint16_t* g = rs.set.gap_pool + (rs.set.gap_base[nb] + (rel & BMB200_DESC_REL_MASK)) * (size_t)kGapUnit + (rel >> 29);
+                const uint16_t* g = gap_block_ptr(rs.set.gap_pool + rs.set.gap_base[nb] * (size_t)kGapUnit, d);
                 c += gap_count_from(g, f >> 16, k << 9, in);
             }
             r += c;
@@ -505,7 +504,7 @@ __global__ void __launch_bounds__(256) rs_select_kernel(const RsView rs, const u
                 }
                 bit = (16u * k + widx) * 32u + __fns(wsel, 0, (int)need);
             } else {
-                const uint16_t* g = rs.set.gap_pool + (rs.set.gap_base[nb] + (rel & BMB200_DESC_REL_MASK)) * (size_t)kGapUnit + (rel >> 29);
+                const uint16_t* g = gap_block_ptr(rs.set.gap_pool + rs.set.gap_base[nb] * (size_t)kGapUnit, d);
                 const uint32_t firstv = g[0] & 1u;
                 uint32_t kr = ent >> 16, s = k << 9;
                 for (;; ++kr) {

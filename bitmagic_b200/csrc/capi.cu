@@ -1230,6 +1230,83 @@ static int result_alloc(bmb200_ctx* ctx, uint32_t n_cols, uint32_t n_groups, boo
     return BMB200_OK;
 }
 
+// the column range [nb_from, nb_to) of a launch over `set` (nb_to = 0: to its last column) -> *cols
+static int col_range(const bmb200_set* set, uint32_t nb_from, uint32_t nb_to, uint32_t* cols)
+{
+    if (!nb_to) nb_to = set->v.n_blocks;
+    if (nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
+    *cols = nb_to - nb_from;
+    return BMB200_OK;
+}
+
+// a scan's planes [plane0, plane0 + n_planes) and its universe vector (0xffffffff = none) lie inside `set`
+static int plane_range(const bmb200_set* set, uint32_t plane0, uint32_t n_planes, uint32_t universe)
+{
+    if ((uint64_t)plane0 + n_planes > set->v.n_vec) return BMB200_ERR_RANGE;
+    if (universe != 0xffffffffu && universe >= set->v.n_vec) return BMB200_ERR_RANGE;
+    return BMB200_OK;
+}
+
+// what the OR buffer of a recycled result means to a launch: the scans, binop and the rank paths refuse a result that has one;
+// an aggregation leaves it unused (kOrKeep) or needs one (kOrNeed, BMB200_F_OR_TARGET)
+enum OrRule { kOrRefuse, kOrKeep, kOrNeed };
+
+// *inout is recycled when it has the shape asked for (n_cols columns in n_groups groups, stored blocks and GAP forms when asked
+// for, an OR buffer as or_rule says), else freed and replaced by a new result -> *out.  The result is then marked for this
+// launch: blocks stored or not, compress mode, GAP forms not written yet, the OR buffer filled by it or not.
+static int prepare_result(bmb200_ctx* ctx, uint32_t n_cols, uint32_t n_groups, bool blocks, bool gaps, bool compress, OrRule or_rule,
+                          bmb200_result** inout, bmb200_result** out)
+{
+    bmb200_result* r = *inout;
+    if (r && (r->ctx != ctx || r->n_cols != n_cols || r->n_groups != n_groups || (blocks && !r->blocks) || (gaps && !r->gaps) ||
+              (or_rule == kOrRefuse && r->or_blocks) || (or_rule == kOrNeed && !r->or_blocks))) {
+        bmb200_result_free(r); r = nullptr; *inout = nullptr;
+    }
+    if (!r) {
+        int rc = result_alloc(ctx, n_cols, n_groups, blocks, gaps, or_rule == kOrNeed, &r);
+        if (rc) return rc;
+    }
+    r->has_blocks = blocks; r->compress = compress; r->gaps_ready = false; r->has_or = or_rule == kOrNeed;
+    *out = r;
+    return BMB200_OK;
+}
+
+// a call that fails after prepare_result: a result allocated for it (*inout still null) must not leak, a recycled one stays
+// with the caller
+static int bail(bmb200_result* r, bmb200_result* const* inout, int rc)
+{
+    if (!*inout) bmb200_result_free(r);
+    return rc;
+}
+
+// before a launch that claims work items and counts into r: zeroes the work counter and the n_groups totals.  An error is
+// reported under `what`.
+static int launch_prologue(bmb200_ctx* ctx, bmb200_result* r, bmb200_result** inout, uint32_t n_groups, const char* what)
+{
+    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8 * (size_t)n_groups, ctx->stream);
+    if (e != cudaSuccess) { ctx->last_err = std::string(what) + ": " + cudaGetErrorString(e); return bail(r, inout, BMB200_ERR_CUDA); }
+    return BMB200_OK;
+}
+
+// after the last launch into r: r is published to *inout, and with gaps_written (the kernel epilogue converted the stored
+// blocks) its GAP forms are ready
+static int launch_epilogue(bmb200_ctx* ctx, bmb200_result* r, bmb200_result** inout, bool gaps_written)
+{
+    const int rc = after_launch(ctx);
+    if (rc) return bail(r, inout, rc);
+    *inout = r;
+    if (gaps_written) r->gaps_ready = true;
+    return BMB200_OK;
+}
+
+// CTAs of a launch over `items` work items: ctas_per_sm per SM, no more than there are items
+static uint32_t work_grid(const bmb200_ctx* ctx, uint64_t items, int ctas_per_sm)
+{
+    const uint64_t g = (uint64_t)ctx->sm_count * (uint64_t)ctas_per_sm;
+    return (uint32_t)(g < items ? g : items);
+}
+
 // dynamic shared memory per aggregation kernel: depends on its static size (the live mask is 8 KB aligned in the shared window)
 extern "C++" {
 template <typename KFn>
@@ -1563,8 +1640,9 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
 {
     if (!ctx || !set || !a || !inout || set->ctx != ctx || !a->n_groups || !a->offsets) return BMB200_ERR_BADARG;
     if (a->op < BMB200_OP_OR || a->op > BMB200_OP_SHIFT_R_AND) return BMB200_ERR_BADARG;
-    const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
-    if (a->nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
+    uint32_t cols = 0;
+    int rc = col_range(set, a->nb_from, a->nb_to, &cols);
+    if (rc) return rc;
     const uint32_t ng = a->n_groups;
     const size_t nmem = a->offsets[2 * (size_t)ng];
     for (uint32_t k = 0; k < 2 * ng; ++k) if (a->offsets[k] > a->offsets[k + 1]) return BMB200_ERR_BADARG;
@@ -1572,25 +1650,16 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     for (size_t k = 0; k < nmem; ++k) if (a->members[k] >= set->v.n_vec) return BMB200_ERR_RANGE;
     if (a->op == BMB200_OP_SHIFT_R_AND)
         for (uint32_t g = 0; g < ng; ++g) if (a->offsets[2 * g + 1] - a->offsets[2 * g] > 65536u) return BMB200_ERR_RANGE;
-    const uint64_t tot_cols = (uint64_t)(nb_to - a->nb_from) * ng;
+    const uint64_t tot_cols = (uint64_t)cols * ng;
     if (tot_cols > 0x7fffffffull) return BMB200_ERR_RANGE;
     CU(cudaSetDevice(ctx->device));
-    const uint32_t cols = nb_to - a->nb_from, n_cols = (uint32_t)tot_cols;
+    const uint32_t n_cols = (uint32_t)tot_cols;
     const bool store = !(a->flags & BMB200_F_COUNT_ONLY);
     const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
     const bool or_target = (a->flags & BMB200_F_OR_TARGET) != 0;
 
-    bmb200_result* r = *inout;
-    if (r && (r->ctx != ctx || r->n_cols != n_cols || r->n_groups != ng || (store && !r->blocks) ||
-              (store && compress && !r->gaps) || (or_target && !r->or_blocks))) {
-        bmb200_result_free(r); r = nullptr; *inout = nullptr;
-    }
-    if (!r) {
-        int rc = result_alloc(ctx, n_cols, ng, store, store && compress, or_target, &r);
-        if (rc) return rc;
-    }
-    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
-    r->has_blocks = store; r->compress = compress; r->gaps_ready = false; r->has_or = or_target;
+    bmb200_result* r = nullptr;
+    if ((rc = prepare_result(ctx, n_cols, ng, store, store && compress, compress, or_target ? kOrNeed : kOrKeep, inout, &r))) return rc;
     if (r->total_inline && ctx->comm.comm) {
         r->xflip = (r->xflip + 1u) % (uint32_t)CommState::kSlots;
         r->popcnt = r->popcnt_base + (size_t)r->xflip * r->xstride;
@@ -1600,21 +1669,16 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
     }
 
     // member ids + offsets -> device (pinned staging keeps the copy asynchronous; skipped when unchanged)
-    int rc = stage_group(ctx, a->members, nmem, a->offsets, 2 * (size_t)ng + 1, true);
-    if (rc) return bail(rc);
-    cudaError_t ce = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
-    if (ce == cudaSuccess) ce = cudaMemsetAsync(r->total, 0, 8 * (size_t)ng, ctx->stream);
-    if (ce == cudaSuccess && or_target) ce = cudaMemsetAsync(r->or_blocks, 0, (size_t)cols * BMB200_BLOCK_BYTES, ctx->stream);
-    if (ce != cudaSuccess) { ctx->last_err = std::string("aggregate: ") + cudaGetErrorString(ce); return bail(BMB200_ERR_CUDA); }
+    if ((rc = stage_group(ctx, a->members, nmem, a->offsets, 2 * (size_t)ng + 1, true))) return bail(r, inout, rc);
+    if ((rc = launch_prologue(ctx, r, inout, ng, "aggregate"))) return rc;
+    cudaError_t ce = or_target ? cudaMemsetAsync(r->or_blocks, 0, (size_t)cols * BMB200_BLOCK_BYTES, ctx->stream) : cudaSuccess;
+    if (ce != cudaSuccess) { ctx->last_err = std::string("aggregate: ") + cudaGetErrorString(ce); return bail(r, inout, BMB200_ERR_CUDA); }
 
     AggParams p = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
     p.group = ctx->d_group; p.goff = ctx->d_group + nmem; p.n_groups = ng;
     p.or_blocks = or_target ? r->or_blocks : nullptr;
     set_agg_attrs(ctx, &ce);
-    if (ce != cudaSuccess) { ctx->last_err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(ce); return bail(BMB200_ERR_CUDA); }
-    const uint32_t sms = (uint32_t)ctx->sm_count;
-    uint32_t grid = sms * (uint32_t)ctx->agg_ctas_per_sm;
-    if (grid > n_cols) grid = n_cols;
+    if (ce != cudaSuccess) { ctx->last_err = std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(ce); return bail(r, inout, BMB200_ERR_CUDA); }
     RunLists rl{};
     Coverage cv{};
     if (ctx->agg_pipeline && ctx->gap_mode == 0 && set->n_gap_units && whole_set(a, set->v.n_vec) &&
@@ -1625,19 +1689,15 @@ int bmb200_aggregate_batch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_
         // OR stays on agg_kernel: its whole-set workloads measured at par or slower through the ring (DESIGN §3.1a)
         const bool cov = cv.slot != nullptr;
         p.dyn_bytes = (uint32_t)ctx->pipe_dyn[cov];
-        const uint32_t pctas = sms * (uint32_t)ctx->pipe_ctas_per_sm[cov];
-        const uint32_t pgrid = pctas < n_cols ? pctas : n_cols;
+        const uint32_t pgrid = work_grid(ctx, n_cols, ctx->pipe_ctas_per_sm[cov]);
         if (cov) agg_pipe_kernel<true><<<pgrid, kPipeThreads, ctx->pipe_dyn[1], ctx->stream>>>(p, rl, cv);
         else agg_pipe_kernel<false><<<pgrid, kPipeThreads, ctx->pipe_dyn[0], ctx->stream>>>(p, rl, cv);
     } else if (a->op == BMB200_OP_SHIFT_R_AND) {
-        shift_and_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p);
+        shift_and_kernel<<<work_grid(ctx, n_cols, ctx->agg_ctas_per_sm), kAggThreads, 0, ctx->stream>>>(p);
     } else {
-        launch_agg_kernel(ctx, a->op, grid, p);
+        launch_agg_kernel(ctx, a->op, work_grid(ctx, n_cols, ctx->agg_ctas_per_sm), p);
     }
-    if ((rc = after_launch(ctx))) return bail(rc);
-    *inout = r;
-    if (store && compress) r->gaps_ready = true;      // bit -> GAP conversion is fused into the kernel epilogue
-    return BMB200_OK;
+    return launch_epilogue(ctx, r, inout, store && compress);      // bit -> GAP conversion is fused into the kernel epilogue
 }
 
 int bmb200_aggregate(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_agg_args* a, bmb200_result** inout)
@@ -1660,42 +1720,35 @@ int bmb200_binop(bmb200_ctx* ctx, const bmb200_set* set, int op, uint32_t va, ui
     if (op != BMB200_OP_OR && op != BMB200_OP_AND && op != BMB200_OP_XOR && op != BMB200_OP_SUB) return BMB200_ERR_BADARG;
     if (flags & (BMB200_F_COUNT_ONLY | BMB200_F_OR_TARGET)) return BMB200_ERR_BADARG;
     if (va >= set->v.n_vec || vb >= set->v.n_vec) return BMB200_ERR_RANGE;
-    if (!nb_to) nb_to = set->v.n_blocks;
-    if (nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
+    uint32_t cols = 0;
+    int rc = col_range(set, nb_from, nb_to, &cols);
+    if (rc) return rc;
     CU(cudaSetDevice(ctx->device));
-    const uint32_t cols = nb_to - nb_from;
     const bool compress = (flags & BMB200_F_OPT_COMPRESS) != 0;
-    bmb200_result* r = *inout;
-    if (r && (r->ctx != ctx || r->n_cols != cols || r->n_groups != 1u || !r->blocks || !r->gaps || r->or_blocks)) { bmb200_result_free(r); r = nullptr; *inout = nullptr; }
-    if (!r) { int rc = result_alloc(ctx, cols, 1u, true, true, false, &r); if (rc) return rc; }
-    r->has_blocks = true; r->compress = true; r->gaps_ready = true;      // GAP-kind results exist in every opt mode (GAP x GAP merges, cloned GAP blocks)
-    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };
+    bmb200_result* r = nullptr;
+    if ((rc = prepare_result(ctx, cols, 1u, true, true, true, kOrRefuse, inout, &r))) return rc;
+    r->gaps_ready = true;      // GAP-kind results exist in every opt mode (GAP x GAP merges, cloned GAP blocks)
     // the two member ids (a, b) -> device, through the pinned group staging buffer like every aggregate
     const uint32_t mem[2] = {va, vb};
     const uint32_t off[3] = {0u, op == BMB200_OP_SUB ? 1u : 2u, 2u};
-    int rc = stage_group(ctx, mem, 2, off, 3, false);
-    if (rc) return bail(rc);
-    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
-    if (e == cudaSuccess) set_agg_attrs(ctx, &e);
+    if ((rc = stage_group(ctx, mem, 2, off, 3, false))) return bail(r, inout, rc);
+    if ((rc = launch_prologue(ctx, r, inout, 1u, "binop"))) return rc;
+    cudaError_t e = cudaSuccess;
+    set_agg_attrs(ctx, &e);
     if (e == cudaSuccess && !ctx->merge_attr_set) { e = cudaFuncSetAttribute(gap_merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMergeSmem); ctx->merge_attr_set = (e == cudaSuccess); }
-    if (e != cudaSuccess) { ctx->last_err = std::string("binop: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
+    if (e != cudaSuccess) { ctx->last_err = std::string("binop: ") + cudaGetErrorString(e); return bail(r, inout, BMB200_ERR_CUDA); }
     const uint32_t bop = op == BMB200_OP_OR ? BINOP_OR : op == BMB200_OP_AND ? BINOP_AND : op == BMB200_OP_XOR ? BINOP_XOR : BINOP_SUB;
     // 1) GAP x GAP columns: merged as run lists (never expanded)
     MergeParams mp{};
     mp.set = set->v; mp.va = va; mp.vb = vb; mp.op = bop; mp.nb_from = nb_from; mp.n_cols = cols;
     mp.kind = r->kind; mp.popcnt = r->popcnt; mp.digest = r->digest; mp.nruns = r->nruns; mp.gaps = r->gaps; mp.total = r->total;
-    uint32_t mgrid = (cols + kMergeWarps - 1) / kMergeWarps; const uint32_t mmax = (uint32_t)ctx->sm_count * 8u; if (mgrid > mmax) mgrid = mmax;
-    gap_merge_kernel<<<mgrid, kMergeWarps * 32, kMergeSmem, ctx->stream>>>(mp);
-    if ((rc = after_launch(ctx))) return bail(rc);
+    gap_merge_kernel<<<work_grid(ctx, (cols + kMergeWarps - 1) / kMergeWarps, 8), kMergeWarps * 32, kMergeSmem, ctx->stream>>>(mp);
+    if ((rc = after_launch(ctx))) return bail(r, inout, rc);
     // 2) every other pairing (and merged blocks that outgrew the GAP format) through the block kernel, kinds by binop_rule
     AggParams p = agg_params(ctx, set, r, nb_from, cols, compress, true);
     p.group = ctx->d_group; p.goff = ctx->d_group + 2; p.n_groups = 1; p.binary = 1u + bop;
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm); if (grid > cols) grid = cols;
-    launch_agg_kernel(ctx, op == BMB200_OP_SUB ? BMB200_OP_AND_SUB : op, grid, p);
-    if ((rc = after_launch(ctx))) return bail(rc);
-    *inout = r;
-    return BMB200_OK;
+    launch_agg_kernel(ctx, op == BMB200_OP_SUB ? BMB200_OP_AND_SUB : op, work_grid(ctx, cols, ctx->agg_ctas_per_sm), p);
+    return launch_epilogue(ctx, r, inout, false);
 }
 
 // bmb200_scan with BMB200_SCAN_IN: the list -> sorted, unique codes below 2^n_planes in a device buffer of its own, then one
@@ -1705,11 +1758,9 @@ static int scan_in(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_arg
     if (!a->n_planes || a->n_planes > 64u) return BMB200_ERR_BADARG;
     if (a->flags & ~(BMB200_F_COUNT_ONLY | BMB200_F_OPT_COMPRESS | BMB200_F_SIGNED)) return BMB200_ERR_BADARG;
     if (a->n_values > BMB200_SCAN_IN_MAX_VALUES) return BMB200_ERR_RANGE;
-    if ((uint64_t)a->plane0 + a->n_planes > set->v.n_vec) return BMB200_ERR_RANGE;
-    if (a->universe != 0xffffffffu && a->universe >= set->v.n_vec) return BMB200_ERR_RANGE;
-    const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
-    if (a->nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
-    const uint32_t cols = nb_to - a->nb_from;
+    uint32_t cols = 0;
+    int rc = plane_range(set, a->plane0, a->n_planes, a->universe);
+    if (rc || (rc = col_range(set, a->nb_from, a->nb_to, &cols))) return rc;
     const bool sgn = (a->flags & BMB200_F_SIGNED) != 0;
     std::vector<uint64_t> codes;
     try { codes.reserve(a->n_values); } catch (...) { return BMB200_ERR_BADALLOC; }
@@ -1725,32 +1776,21 @@ static int scan_in(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_arg
     const bool store = !(a->flags & BMB200_F_COUNT_ONLY);
     const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
 
-    bmb200_result* r = *inout;
-    if (r && (r->ctx != ctx || r->n_cols != cols || r->n_groups != 1u || (store && !r->blocks) ||
-              (store && compress && !r->gaps) || r->or_blocks)) {
-        bmb200_result_free(r); r = nullptr; *inout = nullptr;
-    }
-    if (!r) {
-        int rc = result_alloc(ctx, cols, 1u, store, store && compress, false, &r);
-        if (rc) return rc;
-    }
-    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
-    r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
-
+    bmb200_result* r = nullptr;
+    if ((rc = prepare_result(ctx, cols, 1u, store, store && compress, compress, kOrRefuse, inout, &r))) return rc;
     uint64_t* d_codes = nullptr;
-    int rc = pool_dev(ctx, kDevScanIn, 8 * std::max<size_t>(codes.size(), 1), (void**)&d_codes);
-    if (rc) return bail(rc);
+    if ((rc = pool_dev(ctx, kDevScanIn, 8 * std::max<size_t>(codes.size(), 1), (void**)&d_codes))) return bail(r, inout, rc);
     // a pageable source: the call returns once the codes are staged, so the vector may go out of scope
     cudaError_t e = codes.empty() ? cudaSuccess : cudaMemcpyAsync(d_codes, codes.data(), 8 * codes.size(), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
+    if (e != cudaSuccess) { ctx->last_err = std::string("scan_in: ") + cudaGetErrorString(e); return bail(r, inout, BMB200_ERR_CUDA); }
+    if ((rc = launch_prologue(ctx, r, inout, 1u, "scan_in"))) return rc;
     const size_t smem = scan_in_smem(a->n_planes);
-    if (e == cudaSuccess && !ctx->scan_in_attr_set) {
+    if (!ctx->scan_in_attr_set) {
         e = cudaFuncSetAttribute(scan_in_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_in_smem(64));
         if (e == cudaSuccess) e = cudaFuncSetAttribute(scan_in_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scan_in_smem(64));
         ctx->scan_in_attr_set = (e == cudaSuccess);
     }
-    if (e != cudaSuccess) { ctx->last_err = std::string("scan_in: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
+    if (e != cudaSuccess) { ctx->last_err = std::string("scan_in: ") + cudaGetErrorString(e); return bail(r, inout, BMB200_ERR_CUDA); }
 
     ScanInParams sp{};
     sp.out = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
@@ -1760,14 +1800,8 @@ static int scan_in(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_arg
     sp.bucket = sp.n_codes > kInStage ? (sp.n_codes + kInStage - 1u) / kInStage : 0u;     // splitters: one per bucket
     sp.n_stage = sp.bucket ? (sp.n_codes + sp.bucket - 1u) / sp.bucket : sp.n_codes;
     sp.codes = d_codes;
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
-    if (grid > cols) grid = cols;
-    if (a->n_planes > 32u) scan_in_kernel<true><<<grid, kAggThreads, smem, ctx->stream>>>(sp);
-    else scan_in_kernel<false><<<grid, kAggThreads, smem, ctx->stream>>>(sp);
-    if ((rc = after_launch(ctx))) return bail(rc);
-    *inout = r;
-    if (store && compress) r->gaps_ready = true;
-    return BMB200_OK;
+    (a->n_planes > 32u ? scan_in_kernel<true> : scan_in_kernel<false>)<<<work_grid(ctx, cols, ctx->agg_ctas_per_sm), kAggThreads, smem, ctx->stream>>>(sp);
+    return launch_epilogue(ctx, r, inout, store && compress);
 }
 
 // bmb200_sv_mismatch / bmb200_sv_first_mismatch: argument checks shared by both forms; *cols = columns of the launch
@@ -1778,10 +1812,7 @@ static int mismatch_check(const bmb200_set* set, const bmb200_mismatch_args* a, 
     if (a->n_planes_a > 64u || a->n_planes_b > 64u) return BMB200_ERR_BADARG;
     if ((uint64_t)a->plane0_a + a->n_planes_a > M || (uint64_t)a->plane0_b + a->n_planes_b > M) return BMB200_ERR_BADARG;
     if ((a->not_null_a != kNone && a->not_null_a >= M) || (a->not_null_b != kNone && a->not_null_b >= M)) return BMB200_ERR_BADARG;
-    const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
-    if (a->nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
-    *cols = nb_to - a->nb_from;
-    return BMB200_OK;
+    return col_range(set, a->nb_from, a->nb_to, cols);
 }
 
 static MismatchParams mismatch_params(const bmb200_mismatch_args* a)
@@ -1804,30 +1835,14 @@ int bmb200_sv_mismatch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_mism
     const bool store = !(a->flags & BMB200_F_COUNT_ONLY);
     const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
 
-    bmb200_result* r = *inout;
-    if (r && (r->ctx != ctx || r->n_cols != cols || r->n_groups != 1u || (store && !r->blocks) ||
-              (store && compress && !r->gaps) || r->or_blocks)) {
-        bmb200_result_free(r); r = nullptr; *inout = nullptr;
-    }
-    if (!r) {
-        if ((rc = result_alloc(ctx, cols, 1u, store, store && compress, false, &r))) return rc;
-    }
-    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
-    r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
-    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
-    if (e != cudaSuccess) { ctx->last_err = std::string("sv_mismatch: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
-
+    bmb200_result* r = nullptr;
+    if ((rc = prepare_result(ctx, cols, 1u, store, store && compress, compress, kOrRefuse, inout, &r))) return rc;
+    if ((rc = launch_prologue(ctx, r, inout, 1u, "sv_mismatch"))) return rc;
     MismatchParams mp = mismatch_params(a);
     mp.out = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
     mp.out.n_groups = 1u;
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
-    if (grid > cols) grid = cols;
-    mismatch_kernel<false><<<grid, kAggThreads, 0, ctx->stream>>>(mp);
-    if ((rc = after_launch(ctx))) return bail(rc);
-    *inout = r;
-    if (store && compress) r->gaps_ready = true;
-    return BMB200_OK;
+    mismatch_kernel<false><<<work_grid(ctx, cols, ctx->agg_ctas_per_sm), kAggThreads, 0, ctx->stream>>>(mp);
+    return launch_epilogue(ctx, r, inout, store && compress);
 }
 
 int bmb200_sv_first_mismatch(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_mismatch_args* a, uint64_t* pos, int* found)
@@ -1846,9 +1861,7 @@ int bmb200_sv_first_mismatch(bmb200_ctx* ctx, const bmb200_set* set, const bmb20
     mp.out.set = set->v; mp.out.nb_from = a->nb_from; mp.out.n_cols = cols; mp.out.n_groups = 1u;
     mp.out.work_counter = ctx->d_work;
     mp.first = d_first;
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
-    if (grid > cols) grid = cols;
-    mismatch_kernel<true><<<grid, kAggThreads, 0, ctx->stream>>>(mp);
+    mismatch_kernel<true><<<work_grid(ctx, cols, ctx->agg_ctas_per_sm), kAggThreads, 0, ctx->stream>>>(mp);
     if ((rc = after_launch(ctx))) return rc;
     unsigned long long h = ~0ull;
     CU(cudaMemcpyAsync(&h, d_first, 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1857,6 +1870,19 @@ int bmb200_sv_first_mismatch(bmb200_ctx* ctx, const bmb200_set* set, const bmb20
     *found = h != ~0ull;
     return BMB200_OK;
 }
+
+// scan_kernel<VG, MODE, ENC> by [ENC][MODE][VG / 2: 1, 2, 4 values per pass]; null where there is none (only find_eq groups 4
+// values, float vectors have no find_eq)
+static void (*const kScanKernels[3][3][3])(const ScanParams) = {
+    {{scan_kernel<1, 0, kEncUnsigned>, scan_kernel<2, 0, kEncUnsigned>, scan_kernel<4, 0, kEncUnsigned>},
+     {scan_kernel<1, 1, kEncUnsigned>, scan_kernel<2, 1, kEncUnsigned>, nullptr},
+     {scan_kernel<1, 2, kEncUnsigned>, scan_kernel<2, 2, kEncUnsigned>, nullptr}},
+    {{scan_kernel<1, 0, kEncS2u>, scan_kernel<2, 0, kEncS2u>, scan_kernel<4, 0, kEncS2u>},
+     {scan_kernel<1, 1, kEncS2u>, scan_kernel<2, 1, kEncS2u>, nullptr},
+     {scan_kernel<1, 2, kEncS2u>, scan_kernel<2, 2, kEncS2u>, nullptr}},
+    {{nullptr, nullptr, nullptr},
+     {scan_kernel<1, 1, kEncFloat>, scan_kernel<2, 1, kEncFloat>, nullptr},
+     {scan_kernel<1, 2, kEncFloat>, scan_kernel<2, 2, kEncFloat>, nullptr}}};
 
 int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* a, bmb200_result** inout)
 {
@@ -1870,11 +1896,10 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
     if (fl)
         for (size_t k = 0; k < (size_t)a->n_values * (two ? 2 : 1); ++k)
             if (a->values[k] >> 32) return BMB200_ERR_BADARG;
-    if ((uint64_t)a->plane0 + a->n_planes > set->v.n_vec) return BMB200_ERR_RANGE;
-    if (a->universe != 0xffffffffu && a->universe >= set->v.n_vec) return BMB200_ERR_RANGE;
-    const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
-    if (a->nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
-    const uint32_t cols = nb_to - a->nb_from, nv = a->n_values;
+    uint32_t cols = 0;
+    int rc = plane_range(set, a->plane0, a->n_planes, a->universe);
+    if (rc || (rc = col_range(set, a->nb_from, a->nb_to, &cols))) return rc;
+    const uint32_t nv = a->n_values;
     const uint64_t tot_cols = (uint64_t)cols * nv;
     if (tot_cols > 0x7fffffffull) return BMB200_ERR_RANGE;
     CU(cudaSetDevice(ctx->device));
@@ -1882,25 +1907,12 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
     const bool store = !(a->flags & BMB200_F_COUNT_ONLY);
     const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
 
-    bmb200_result* r = *inout;
-    if (r && (r->ctx != ctx || r->n_cols != n_cols || r->n_groups != nv || (store && !r->blocks) ||
-              (store && compress && !r->gaps) || r->or_blocks)) {
-        bmb200_result_free(r); r = nullptr; *inout = nullptr;
-    }
-    if (!r) {
-        int rc = result_alloc(ctx, n_cols, nv, store, store && compress, false, &r);
-        if (rc) return rc;
-    }
-    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
-    r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
-
+    bmb200_result* r = nullptr;
+    if ((rc = prepare_result(ctx, n_cols, nv, store, store && compress, compress, kOrRefuse, inout, &r))) return rc;
     // search values -> device through the (pinned) group staging buffer, 2 words per value
     const size_t nvals = (size_t)nv * (two ? 2 : 1);
-    int rc = stage_group(ctx, reinterpret_cast<const uint32_t*>(a->values), 2 * nvals, nullptr, 0, false);
-    if (rc) return bail(rc);
-    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8 * (size_t)nv, ctx->stream);
-    if (e != cudaSuccess) { ctx->last_err = std::string("scan: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
+    if ((rc = stage_group(ctx, reinterpret_cast<const uint32_t*>(a->values), 2 * nvals, nullptr, 0, false))) return bail(r, inout, rc);
+    if ((rc = launch_prologue(ctx, r, inout, nv, "scan"))) return rc;
 
     ScanParams sp{};
     sp.out = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
@@ -1911,25 +1923,11 @@ int bmb200_scan(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_args* 
     // RANGE_OPEN four (2 values); single searches use the narrow kernels
     const int mode = a->pred == BMB200_SCAN_EQ ? 0 : two ? 2 : 1;
     const uint32_t vg = nv == 1 ? 1u : (mode == 0 && nv >= 4 ? 4u : 2u);
-    const uint64_t items = (uint64_t)cols * ((nv + vg - 1) / vg);
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
-    if (grid > items) grid = (uint32_t)items;
     // BMB200_F_SIGNED selects the signed instantiations (s2u planes, int64 values), BMB200_F_FLOAT the float ones (sign +
-    // magnitude planes, float bits; no find_eq, so MODE 1 / 2 only), with the same launch shapes
-    #define BMB200_SCAN_LAUNCH(VG, MODE) \
-        do { if (a->flags & BMB200_F_SIGNED) scan_kernel<VG, MODE, kEncS2u><<<grid, kAggThreads, 0, ctx->stream>>>(sp); \
-             else scan_kernel<VG, MODE><<<grid, kAggThreads, 0, ctx->stream>>>(sp); } while (0)
-    #define BMB200_SCAN_LAUNCH_F(VG, MODE) \
-        do { if (fl) scan_kernel<VG, MODE, kEncFloat><<<grid, kAggThreads, 0, ctx->stream>>>(sp); else BMB200_SCAN_LAUNCH(VG, MODE); } while (0)
-    if (mode == 0)      { if (vg == 4) BMB200_SCAN_LAUNCH(4, 0); else if (vg == 2) BMB200_SCAN_LAUNCH(2, 0); else BMB200_SCAN_LAUNCH(1, 0); }
-    else if (mode == 1) { if (vg == 2) BMB200_SCAN_LAUNCH_F(2, 1); else BMB200_SCAN_LAUNCH_F(1, 1); }
-    else                { if (vg == 2) BMB200_SCAN_LAUNCH_F(2, 2); else BMB200_SCAN_LAUNCH_F(1, 2); }
-    #undef BMB200_SCAN_LAUNCH_F
-    #undef BMB200_SCAN_LAUNCH
-    if ((rc = after_launch(ctx))) return bail(rc);
-    *inout = r;
-    if (store && compress) r->gaps_ready = true;
-    return BMB200_OK;
+    // magnitude planes, float bits), with the same launch shapes
+    const int enc = fl ? kEncFloat : (a->flags & BMB200_F_SIGNED) ? kEncS2u : kEncUnsigned;
+    kScanKernels[enc][mode][vg >> 1]<<<work_grid(ctx, (uint64_t)cols * ((nv + vg - 1) / vg), ctx->agg_ctas_per_sm), kAggThreads, 0, ctx->stream>>>(sp);
+    return launch_epilogue(ctx, r, inout, store && compress);
 }
 
 int bmb200_scan_str(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_str_args* a, bmb200_result** inout)
@@ -1937,11 +1935,10 @@ int bmb200_scan_str(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_st
     if (!ctx || !set || !a || !inout || set->ctx != ctx || !a->strs || !a->stride || !a->n_values) return BMB200_ERR_BADARG;
     if (!a->n_planes || a->n_planes > kStrMaxPlanes) return BMB200_ERR_BADARG;
     if (a->flags & ~(BMB200_F_COUNT_ONLY | BMB200_F_OPT_COMPRESS | BMB200_F_STR_PREFIX)) return BMB200_ERR_BADARG;
-    if ((uint64_t)a->plane0 + a->n_planes > set->v.n_vec) return BMB200_ERR_RANGE;
-    if (a->universe != 0xffffffffu && a->universe >= set->v.n_vec) return BMB200_ERR_RANGE;
-    const uint32_t nb_to = a->nb_to ? a->nb_to : set->v.n_blocks;
-    if (a->nb_from >= nb_to || nb_to > set->v.n_blocks) return BMB200_ERR_RANGE;
-    const uint32_t cols = nb_to - a->nb_from, nv = a->n_values;
+    uint32_t cols = 0;
+    int rc = plane_range(set, a->plane0, a->n_planes, a->universe);
+    if (rc || (rc = col_range(set, a->nb_from, a->nb_to, &cols))) return rc;
+    const uint32_t nv = a->n_values;
     const uint64_t tot_cols = (uint64_t)cols * nv;
     if (tot_cols > 0x7fffffffull) return BMB200_ERR_RANGE;
 
@@ -1974,23 +1971,10 @@ int bmb200_scan_str(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_st
     const bool store = !(a->flags & BMB200_F_COUNT_ONLY);
     const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
 
-    bmb200_result* r = *inout;
-    if (r && (r->ctx != ctx || r->n_cols != n_cols || r->n_groups != nv || (store && !r->blocks) ||
-              (store && compress && !r->gaps) || r->or_blocks)) {
-        bmb200_result_free(r); r = nullptr; *inout = nullptr;
-    }
-    if (!r) {
-        int rc = result_alloc(ctx, n_cols, nv, store, store && compress, false, &r);
-        if (rc) return rc;
-    }
-    auto bail = [&](int rc) { if (!*inout) bmb200_result_free(r); return rc; };   // a freshly allocated result must not leak
-    r->has_blocks = store; r->compress = compress; r->gaps_ready = false;
-
-    int rc = stage_group(ctx, staged.data(), staged.size(), nullptr, 0, false);
-    if (rc) return bail(rc);
-    cudaError_t e = cudaMemsetAsync(ctx->d_work, 0, 4, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8 * (size_t)nv, ctx->stream);
-    if (e != cudaSuccess) { ctx->last_err = std::string("scan_str: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
+    bmb200_result* r = nullptr;
+    if ((rc = prepare_result(ctx, n_cols, nv, store, store && compress, compress, kOrRefuse, inout, &r))) return rc;
+    if ((rc = stage_group(ctx, staged.data(), staged.size(), nullptr, 0, false))) return bail(r, inout, rc);
+    if ((rc = launch_prologue(ctx, r, inout, nv, "scan_str"))) return rc;
 
     StrScanParams sp{};
     sp.out = agg_params(ctx, set, r, a->nb_from, cols, compress, store);
@@ -1999,16 +1983,9 @@ int bmb200_scan_str(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_scan_st
     sp.strs = ctx->d_group;
     // queries per pass as for find_eq: 4 when the batch has them, single searches on the narrow kernel
     const uint32_t vg = nv == 1 ? 1u : nv >= 4 ? 4u : 2u;
-    const uint64_t items = (uint64_t)cols * ((nv + vg - 1) / vg);
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm);
-    if (grid > items) grid = (uint32_t)items;
-    if (vg == 4) str_scan_kernel<4><<<grid, kAggThreads, 0, ctx->stream>>>(sp);
-    else if (vg == 2) str_scan_kernel<2><<<grid, kAggThreads, 0, ctx->stream>>>(sp);
-    else str_scan_kernel<1><<<grid, kAggThreads, 0, ctx->stream>>>(sp);
-    if ((rc = after_launch(ctx))) return bail(rc);
-    *inout = r;
-    if (store && compress) r->gaps_ready = true;
-    return BMB200_OK;
+    static void (*const kStrScanKernels[3])(const StrScanParams) = {str_scan_kernel<1>, str_scan_kernel<2>, str_scan_kernel<4>};
+    kStrScanKernels[vg >> 1]<<<work_grid(ctx, (uint64_t)cols * ((nv + vg - 1) / vg), ctx->agg_ctas_per_sm), kAggThreads, 0, ctx->stream>>>(sp);
+    return launch_epilogue(ctx, r, inout, store && compress);
 }
 
 int bmb200_result_group_totals(bmb200_result* r, uint64_t* totals, uint32_t n_groups)
@@ -2035,8 +2012,7 @@ int bmb200_result_or_target(bmb200_result* r, bmb200_result** out)
     p.n_groups = 1; p.n_cols = r->cols_per_group; p.compress = r->compress ? 1u : 0u; p.store_blocks = 1u;
     p.blocks = o->blocks; p.popcnt = o->popcnt; p.digest = o->digest; p.nruns = o->nruns; p.kind = o->kind; p.gaps = o->gaps;
     p.total = o->total; p.or_blocks = nullptr;
-    uint32_t grid = (uint32_t)(ctx->sm_count * ctx->agg_ctas_per_sm); if (grid > p.n_cols) grid = p.n_cols;
-    finalize_blocks_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p, r->or_blocks);
+    finalize_blocks_kernel<<<work_grid(ctx, p.n_cols, ctx->agg_ctas_per_sm), kAggThreads, 0, ctx->stream>>>(p, r->or_blocks);
     rc = after_launch(ctx);
     if (rc) { bmb200_result_free(o); return rc; }
     *out = o;
@@ -2621,19 +2597,6 @@ int bmb200_rs_free(bmb200_rs* rs)
 
 /* ------------------------------------------------------------------ rank compression (rank_kernel.cuh) */
 
-// *inout recycled when it has the shape asked for, else freed and replaced (as bmb200_scan does)
-static int rank_result(bmb200_ctx* ctx, uint32_t n_cols, uint32_t n_groups, bool compress, bmb200_result** inout, bmb200_result** out)
-{
-    bmb200_result* r = *inout;
-    if (r && (r->ctx != ctx || r->n_cols != n_cols || r->n_groups != n_groups || !r->blocks || (compress && !r->gaps) || r->or_blocks)) {
-        bmb200_result_free(r); r = nullptr; *inout = nullptr;
-    }
-    if (!r) { int rc = result_alloc(ctx, n_cols, n_groups, true, compress, false, &r); if (rc) return rc; }
-    r->has_blocks = true; r->compress = compress; r->gaps_ready = compress;      // the epilogue writes the GAP form in compress mode
-    *out = r;
-    return BMB200_OK;
-}
-
 int bmb200_rank_decompress(bmb200_ctx* ctx, const bmb200_rs* idx, const bmb200_result* src, uint32_t flags, bmb200_result** inout)
 {
     if (!ctx || !idx || !src || !inout || idx->ctx != ctx || src->ctx != ctx || *inout == src) return BMB200_ERR_BADARG;
@@ -2646,20 +2609,17 @@ int bmb200_rank_decompress(bmb200_ctx* ctx, const bmb200_rs* idx, const bmb200_r
     CU(cudaSetDevice(ctx->device));
     const bool compress = (flags & BMB200_F_OPT_COMPRESS) != 0;
     bmb200_result* r = nullptr;
-    int rc = rank_result(ctx, (uint32_t)tot_cols, src->n_groups, compress, inout, &r);
+    int rc = prepare_result(ctx, (uint32_t)tot_cols, src->n_groups, true, compress, compress, kOrRefuse, inout, &r);
     if (rc) return rc;
-    auto bail = [&](int e) { if (!*inout) bmb200_result_free(r); return e; };
-    if (cudaMemsetAsync(r->total, 0, 8 * (size_t)r->n_groups, ctx->stream) != cudaSuccess) { ctx->last_err = "rank_decompress: memset"; return bail(BMB200_ERR_CUDA); }
+    r->gaps_ready = compress;                             // the epilogue writes the GAP form in compress mode
+    if (cudaMemsetAsync(r->total, 0, 8 * (size_t)r->n_groups, ctx->stream) != cudaSuccess) { ctx->last_err = "rank_decompress: memset"; return bail(r, inout, BMB200_ERR_CUDA); }
     AggParams p{};
     p.n_groups = r->n_groups; p.n_cols = r->n_cols; p.compress = compress ? 1u : 0u; p.store_blocks = 1u;
     p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
     p.total = r->total;
     RankSrc s{src->kind, src->blocks, src->gaps, src->cols_per_group};
-    uint32_t grid = (uint32_t)(ctx->sm_count * kCtasPerSm); if (grid > p.n_cols) grid = p.n_cols;
-    rank_decompress_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p, rs_view(idx), s);
-    if ((rc = after_launch(ctx))) return bail(rc);
-    *inout = r;
-    return BMB200_OK;
+    rank_decompress_kernel<<<work_grid(ctx, p.n_cols, kCtasPerSm), kAggThreads, 0, ctx->stream>>>(p, rs_view(idx), s);
+    return launch_epilogue(ctx, r, inout, false);
 }
 
 int bmb200_rank_compress(bmb200_ctx* ctx, const bmb200_rs* idx, uint32_t src_vec, uint32_t flags, bmb200_result** inout)
@@ -2679,23 +2639,19 @@ int bmb200_rank_compress(bmb200_ctx* ctx, const bmb200_rs* idx, uint32_t src_vec
     int rc = pool_dev(ctx, kDevRankDense, (size_t)cols * BMB200_BLOCK_BYTES, (void**)&dense);
     if (rc) return rc;
     bmb200_result* r = nullptr;
-    if ((rc = rank_result(ctx, cols, 1u, compress, inout, &r))) return rc;
-    auto bail = [&](int e) { if (!*inout) bmb200_result_free(r); return e; };
+    if ((rc = prepare_result(ctx, cols, 1u, true, compress, compress, kOrRefuse, inout, &r))) return rc;
+    r->gaps_ready = compress;                             // the epilogue writes the GAP form in compress mode
     cudaError_t e = cudaMemsetAsync(dense, 0, (size_t)cols * BMB200_BLOCK_BYTES, ctx->stream);
     if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
-    if (e != cudaSuccess) { ctx->last_err = std::string("rank_compress: ") + cudaGetErrorString(e); return bail(BMB200_ERR_CUDA); }
-    uint32_t grid = (uint32_t)(ctx->sm_count * kCtasPerSm); if (grid > idx->n_blocks) grid = idx->n_blocks;
-    rank_compress_scatter_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(rs_view(idx), src_vec, dense);
-    if ((rc = after_launch(ctx))) return bail(rc);
+    if (e != cudaSuccess) { ctx->last_err = std::string("rank_compress: ") + cudaGetErrorString(e); return bail(r, inout, BMB200_ERR_CUDA); }
+    rank_compress_scatter_kernel<<<work_grid(ctx, idx->n_blocks, kCtasPerSm), kAggThreads, 0, ctx->stream>>>(rs_view(idx), src_vec, dense);
+    if ((rc = after_launch(ctx))) return bail(r, inout, rc);
     AggParams p{};
     p.n_groups = 1; p.n_cols = cols; p.compress = compress ? 1u : 0u; p.store_blocks = 1u;
     p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
     p.total = r->total;
-    grid = (uint32_t)(ctx->sm_count * kCtasPerSm); if (grid > cols) grid = cols;
-    finalize_blocks_kernel<<<grid, kAggThreads, 0, ctx->stream>>>(p, dense);
-    if ((rc = after_launch(ctx))) return bail(rc);
-    *inout = r;
-    return BMB200_OK;
+    finalize_blocks_kernel<<<work_grid(ctx, cols, kCtasPerSm), kAggThreads, 0, ctx->stream>>>(p, dense);
+    return launch_epilogue(ctx, r, inout, false);
 }
 
 }  // extern "C"

@@ -27,6 +27,24 @@ struct SetView {
     const uint16_t* gap_pool;
 };
 
+// A GAP descriptor d addresses its block inside the column's GAP segment gseg (gap_pool + gap_base[nb] * kGapUnit): `unit` is
+// the 16-byte arena unit the block is stored in, `pad` the u16 words before the block's header inside that unit.
+struct GapAddr {
+    const uint16_t* unit;
+    uint32_t        pad;
+};
+__device__ __forceinline__ GapAddr gap_block_addr(const uint16_t* gseg, uint32_t d)
+{
+    const uint32_t rel = d >> 2;
+    return {gseg + (size_t)(rel & BMB200_DESC_REL_MASK) * kGapUnit, rel >> 29};
+}
+// the GAP block of descriptor d: its header word, then its run ends
+__device__ __forceinline__ const uint16_t* gap_block_ptr(const uint16_t* gseg, uint32_t d)
+{
+    const GapAddr a = gap_block_addr(gseg, d);
+    return a.unit + a.pad;
+}
+
 // streaming 128-bit load: read-only path, do not allocate in L1 (each bit-block is read once)
 __device__ __forceinline__ uint4 ld_stream_v4(const uint4* p)
 {

@@ -18,7 +18,7 @@
 //     ascending order, so a CTA whose claimed column starts at or after the best position found so far stops: every column
 //     it could still claim starts later.
 #pragma once
-#include "gap_expand.cuh"
+#include "column_walk.cuh"
 
 namespace bmb200 {
 
@@ -66,19 +66,15 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) mismatch_kernel(const
     const bool use_nn = FIRST ? mp.use_null != 0u : (ha || hb);    // FIRST with no_null compares the planes only
     const uint4 kZero = make_uint4(0u, 0u, 0u, 0u), kOnes = make_uint4(~0u, ~0u, ~0u, ~0u);
 
-    uint32_t next = 0;
-    if (tid == 0) next = atomicAdd(p.work_counter, 1u);
+    // FIRST: a column that starts at or after the best position found so far ends the claims
+    auto past_first = [&](uint32_t c) {
+        return FIRST && c < p.n_cols && ((uint64_t)(p.nb_from + c) << 16) >= *(volatile unsigned long long*)mp.first;
+    };
+    WorkClaim claim(p.work_counter);
     for (;;) {
-        __syncthreads();
-        if (tid == 0) {
-            uint32_t c = next;
-            if (FIRST && c < p.n_cols && ((uint64_t)(p.nb_from + c) << 16) >= *(volatile unsigned long long*)mp.first) c = p.n_cols;
-            s_col = c; s_min = 0xffffffffu;
-        }
-        __syncthreads();
-        const uint32_t colx = s_col;
+        const uint32_t colx = claim.next(p.work_counter, s_col, p.n_cols, past_first);
         if (colx >= p.n_cols) break;
-        if (tid == 0) next = atomicAdd(p.work_counter, 1u);
+        if (FIRST && tid == 0) s_min = 0xffffffffu;          // read after the barrier below
         const uint32_t nb = p.nb_from + colx;
         const uint32_t* drow = p.set.desc + (size_t)nb * M;
         if (tid < 64) s_da[tid] = (uint32_t)tid < mp.n_planes_a ? drow[mp.plane0_a + tid] : BMB200_BLK_NULL;
@@ -89,16 +85,8 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) mismatch_kernel(const
         const uint16_t* gseg = p.set.gap_pool + p.set.gap_base[nb] * (size_t)kGapUnit;
         __syncthreads();
 
-        auto load_now = [&](uint32_t d) -> uint4 {           // NULL / FULL / bit; a GAP block is XOR-ed in from its buffer
-            const uint32_t kind = d & 3u;
-            if (kind == BMB200_BLK_BIT) return ld_stream_v4(bseg + (size_t)(d >> 2) * (kBlockWords / 4));
-            return kind == BMB200_BLK_FULL ? kOnes : kZero;
-        };
-        auto expand = [&](uint32_t buf, uint32_t d) {        // XOR the 1-runs of GAP block d into buffer buf, all threads
-            if ((d & 3u) != BMB200_BLK_GAP) return;
-            const uint32_t rel = d >> 2;
-            gap_expand_block(Ks + buf * kBlockWords * 4u, gseg + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29), tid);
-        };
+        // XOR the 1-runs of GAP block d into buffer buf, all threads
+        auto expand = [&](uint32_t buf, uint32_t d) { if ((d & 3u) == BMB200_BLK_GAP) gap_expand_block(Ks + buf * kBlockWords * 4u, gap_block_ptr(gseg, d), tid); };
 
         uint4 D = kZero;
         bool sat = false;                                    // uniform: a NULL / FULL pair filled D
@@ -113,7 +101,7 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) mismatch_kernel(const
                 X[u] = kZero;
                 if (da == db || (ka == kb && ka <= BMB200_BLK_FULL)) continue;           // cannot differ
                 if (ka <= BMB200_BLK_FULL && kb <= BMB200_BLK_FULL) { sat = true; continue; }   // NULL vs FULL
-                X[u] = xor4(load_now(da), load_now(db));
+                X[u] = xor4(block_now(bseg, da), block_now(bseg, db));
                 if (ka == BMB200_BLK_GAP || kb == BMB200_BLK_GAP) gmask |= 1u << u;
             }
             if (sat) break;
@@ -136,17 +124,10 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) mismatch_kernel(const
         }
         if (sat) D = kOnes;
 
-        // NOT-NULL vectors (GAP ones through K[0] / K[1]); NULL descriptors when absent or unused
-        const uint32_t dna = s_nn[0], dnb = s_nn[1];
-        uint4 NA = load_now(dna), NB = load_now(dnb);
-        if ((dna & 3u) == BMB200_BLK_GAP || (dnb & 3u) == BMB200_BLK_GAP) {
-            reinterpret_cast<uint4*>(K[0])[tid] = kZero; reinterpret_cast<uint4*>(K[1])[tid] = kZero;
-            __syncthreads();
-            expand(0u, dna); expand(1u, dnb);
-            __syncthreads();
-            NA = xor4(NA, reinterpret_cast<const uint4*>(K[0])[tid]); NB = xor4(NB, reinterpret_cast<const uint4*>(K[1])[tid]);
-            __syncthreads();
-        }
+        // NOT-NULL vectors; NULL descriptors when absent or unused
+        uint4 NN[2];
+        load_blocks({s_nn[0], s_nn[1]}, NN, bseg, gseg, K);
+        const uint4 NA = NN[0], NB = NN[1];
         const uint64_t b0 = ((uint64_t)nb << 16) + 128u * (uint32_t)tid;
         const uint64_t sa = mp.size_a, sb = mp.size_b;
         if constexpr (!FIRST) {

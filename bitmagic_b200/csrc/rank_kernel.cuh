@@ -18,7 +18,7 @@
 // than a loop over the set bits of the mask: it costs the same ~5 rounds whatever the density, while a loop would run every lane
 // of a warp as long as its densest lane (up to 32 iterations per word, 128 per thread).
 #pragma once
-#include "gap_expand.cuh"
+#include "column_walk.cuh"
 #include "aux_kernels.cuh"
 
 namespace bmb200 {
@@ -102,8 +102,7 @@ __device__ __forceinline__ uint4 rank_block_words(const SetView& s, uint32_t nb,
 }
 __device__ __forceinline__ const uint16_t* rank_gap_ptr(const SetView& s, uint32_t nb, uint32_t d)
 {
-    const uint32_t rel = d >> 2;
-    return s.gap_pool + s.gap_base[nb] * (size_t)kGapUnit + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29);
+    return gap_block_ptr(s.gap_pool + s.gap_base[nb] * (size_t)kGapUnit, d);
 }
 
 // decompress: one CTA per (group, output column nb), grid-stride over p.n_cols = n_groups * n_blocks(NN), group-major.

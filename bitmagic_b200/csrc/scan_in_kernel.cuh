@@ -17,7 +17,7 @@
 // Codes are the stored ones (s2u(x) for signed vectors): the host applies s2u, sorts, de-duplicates and drops codes with bits at
 // or above n_planes, which no element can hold.
 #pragma once
-#include "gap_expand.cuh"
+#include "column_walk.cuh"
 
 namespace bmb200 {
 
@@ -109,15 +109,10 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_in_kernel(const 
     for (uint32_t i = tid; i < sp.n_stage; i += kAggThreads) L[i] = sp.codes[(size_t)i * (sp.bucket ? sp.bucket : 1u)];
     const uint64_t cmin = sp.n_codes ? sp.codes[0] : 0ull, cmax = sp.n_codes ? sp.codes[sp.n_codes - 1] : 0ull;
 
-    uint32_t next = 0;
-    if (tid == 0) next = atomicAdd(p.work_counter, 1u);
+    WorkClaim claim(p.work_counter);
     for (;;) {
-        __syncthreads();
-        if (tid == 0) s_col = next;
-        __syncthreads();
-        const uint32_t colx = s_col;
+        const uint32_t colx = claim.next(p.work_counter, s_col, p.n_cols);
         if (colx >= p.n_cols) break;
-        if (tid == 0) next = atomicAdd(p.work_counter, 1u);
         const uint32_t nb = p.nb_from + colx;
         const uint32_t* drow = p.set.desc + (size_t)nb * M;
         if (tid < (int)np) s_desc[tid] = drow[sp.plane0 + tid];
@@ -159,8 +154,7 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_in_kernel(const 
                     for (uint32_t r = 0; r <= np; ++r) {
                         const uint32_t d = r < np ? s_desc[r] : du;
                         if ((d & 3u) != BMB200_BLK_GAP) continue;
-                        const uint32_t rel = d >> 2;
-                        gap_expand_chunk(rows + r * kInRowStride, gseg + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29), 32u * c0, tid);
+                        gap_expand_chunk(rows + r * kInRowStride, gap_block_ptr(gseg, d), 32u * c0, tid);
                     }
                 }
                 __syncthreads();

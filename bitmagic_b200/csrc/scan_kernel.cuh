@@ -49,7 +49,7 @@
 //   * RANGE_OPEN (find_range_float_unbounded) is gt(a) & lt(b) = GT_a & U & ~(GT_b | EQ_b), two state pairs like RANGE.
 // The float path has no find_eq (the reference has none) and so only the MODE 1 / 2 instantiations.
 #pragma once
-#include "gap_expand.cuh"
+#include "column_walk.cuh"
 
 namespace bmb200 {
 
@@ -166,8 +166,7 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const Sca
         auto load_gap = [&](uint32_t d) -> uint4 {
             K4[tid] = make_uint4(0u, 0u, 0u, 0u);
             __syncthreads();
-            const uint32_t rel = d >> 2;
-            gap_expand_block(Ks, gseg + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29), tid);
+            gap_expand_block(Ks, gap_block_ptr(gseg, d), tid);
             __syncthreads();
             const uint4 r = K4[tid];
             __syncthreads();
@@ -211,10 +210,7 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_kernel(const Sca
                 __syncthreads();
 #pragma unroll
                 for (int u = 0; u < kBatch; ++u)
-                    if ((d[u] & 3u) == BMB200_BLK_GAP) {
-                        const uint32_t rel = d[u] >> 2;
-                        gap_expand_block(Ks + (uint32_t)u * kBlockWords * 4u, gseg + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29), tid);
-                    }
+                    if ((d[u] & 3u) == BMB200_BLK_GAP) gap_expand_block(Ks + (uint32_t)u * kBlockWords * 4u, gap_block_ptr(gseg, d[u]), tid);
                 __syncthreads();
 #pragma unroll
                 for (int u = 0; u < kBatch; ++u)

@@ -15,7 +15,7 @@
 // constants; indexes below 0 fall into block nb - 1 of the same source.  Epilogue = the aggregation kernel's (popcount,
 // digest, run count, kind, bit->GAP); like every AND-type result an empty digest stores nothing (:2617-2632).
 #pragma once
-#include "scan_kernel.cuh"
+#include "column_walk.cuh"
 
 namespace bmb200 {
 
@@ -32,15 +32,10 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) shift_and_kernel(cons
     uint4* K24 = reinterpret_cast<uint4*>(K2);
     const uint32_t Ks = smem_u32(K), K2s = smem_u32(K2);
 
-    uint32_t next_item = 0;
-    if (tid == 0) next_item = atomicAdd(p.work_counter, 1u);
+    WorkClaim claim(p.work_counter);
     for (;;) {
-        __syncthreads();
-        if (tid == 0) s_col = next_item;
-        __syncthreads();
-        const uint32_t item = s_col;
+        const uint32_t item = claim.next(p.work_counter, s_col, p.n_cols * p.n_groups);
         if (item >= p.n_cols * p.n_groups) break;
-        if (tid == 0) next_item = atomicAdd(p.work_counter, 1u);
         const uint32_t colx = item / p.n_groups, grp = item - colx * p.n_groups;
         const uint32_t col = grp * p.n_cols + colx;
         const uint32_t nb = p.nb_from + colx;
@@ -68,8 +63,8 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) shift_and_kernel(cons
                 if (kd == BMB200_BLK_GAP) K4[tid] = make_uint4(0u, 0u, 0u, 0u);
                 if (kp == BMB200_BLK_GAP) K24[tid] = make_uint4(0u, 0u, 0u, 0u);
                 __syncthreads();
-                if (kd == BMB200_BLK_GAP) { const uint32_t rel = d >> 2; gap_expand_block(Ks, gcur + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29), tid); }
-                if (kp == BMB200_BLK_GAP) { const uint32_t rel = dp >> 2; gap_expand_block(K2s, gprev + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29), tid); }
+                if (kd == BMB200_BLK_GAP) gap_expand_block(Ks, gap_block_ptr(gcur, d), tid);
+                if (kp == BMB200_BLK_GAP) gap_expand_block(K2s, gap_block_ptr(gprev, dp), tid);
                 __syncthreads();
             }
             const uint32_t* bc = bcur + (size_t)(d >> 2) * kBlockWords;       // valid when kd == BIT

@@ -23,7 +23,7 @@
 // Up to 4 queries of a column share one pass (VG), plane loads are batched four at a time, GAP planes are expanded through the
 // shared buffers (one pair of barriers per batch), and the result goes through finish_block like every other result.
 #pragma once
-#include "gap_expand.cuh"
+#include "column_walk.cuh"
 
 namespace bmb200 {
 
@@ -101,10 +101,7 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) str_scan_kernel(const
                 __syncthreads();
 #pragma unroll
                 for (int u = 0; u < kStrBatch; ++u)
-                    if ((d[u] & 3u) == BMB200_BLK_GAP) {
-                        const uint32_t rel = d[u] >> 2;
-                        gap_expand_block(Ks + (uint32_t)u * kBlockWords * 4u, gseg() + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29), tid);
-                    }
+                    if ((d[u] & 3u) == BMB200_BLK_GAP) gap_expand_block(Ks + (uint32_t)u * kBlockWords * 4u, gap_block_ptr(gseg(), d[u]), tid);
                 __syncthreads();
 #pragma unroll
                 for (int u = 0; u < kStrBatch; ++u)
@@ -119,8 +116,7 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) str_scan_kernel(const
             if ((du & 3u) == BMB200_BLK_GAP) {
                 reinterpret_cast<uint4*>(K[0])[tid] = make_uint4(0u, 0u, 0u, 0u);
                 __syncthreads();
-                const uint32_t rel = du >> 2;
-                gap_expand_block(Ks, gseg() + (size_t)(rel & kRelMask) * kGapUnit + (rel >> 29), tid);
+                gap_expand_block(Ks, gap_block_ptr(gseg(), du), tid);
                 __syncthreads();
                 U = reinterpret_cast<const uint4*>(K[0])[tid];
                 __syncthreads();
