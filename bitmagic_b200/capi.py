@@ -504,16 +504,48 @@ class DeviceResult:
         self.ctx.check(lib().bmb200_result_fetch_meta(self._h, C.byref(m)), "result_fetch_meta")
         return kind, pop, dig, nr
 
-    def fetch(self):
-        """(kind[n], off[n], bits[n_bit*2048], gaps[n_gap_words]) -- per-vector flat form."""
+    def sizes(self) -> tuple[int, int]:
+        """bmb200_result_sizes -> (BIT blocks, GAP u16 words) of the compacted result."""
         nb, ng = C.c_uint64(0), C.c_uint64(0)
         self.ctx.check(lib().bmb200_result_sizes(self._h, C.byref(nb), C.byref(ng)), "result_sizes")
+        return nb.value, ng.value
+
+    def optimize(self):
+        """bmb200_result_optimize: write the GAP forms of a F_OPT_COMPRESS result (a no-op once they are written)."""
+        self.ctx.check(lib().bmb200_result_optimize(self._h), "result_optimize")
+
+    def fetch(self):
+        """(kind[n], off[n], bits[n_bit*2048], gaps[n_gap_words]) -- per-vector flat form."""
+        nb, ng = self.sizes()
         kind = np.empty(self.n_cols, np.uint8); off = np.empty(self.n_cols, np.uint64)
-        bits = np.empty(nb.value * BLOCK_WORDS, np.uint32); gaps = np.empty(ng.value, np.uint16)
+        bits = np.empty(nb * BLOCK_WORDS, np.uint32); gaps = np.empty(ng, np.uint16)
         self.ctx.check(lib().bmb200_result_fetch(self._h, ptr(kind), ptr(off),
-                                                 ptr(bits) if nb.value else C.c_void_p(0),
-                                                 ptr(gaps) if ng.value else C.c_void_p(0)), "result_fetch")
+                                                 ptr(bits) if nb else C.c_void_p(0),
+                                                 ptr(gaps) if ng else C.c_void_p(0)), "result_fetch")
         return kind, off, bits, gaps
+
+    def fetch_view(self, wait: bool = True):
+        """bmb200_result_fetch_view (wait=False: bmb200_result_fetch_view_async) -> (kind[n], off[n], bits[n_bit*2048],
+        gaps[n_gap_words], n_bit_blocks, n_gap_words, total), the flat form of fetch() and the cardinality over all groups.
+        wait=True returns copies.  wait=False returns numpy views over pinned memory the context owns: bits / gaps of column c
+        are valid once fetch_wait(c) has returned, and all of it only until the next view on the context, so copy what you keep."""
+        k, o, b, g = C.c_void_p(0), C.c_void_p(0), C.c_void_p(0), C.c_void_p(0)
+        nb, ng, tot = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        fn, what = (lib().bmb200_result_fetch_view, "result_fetch_view") if wait else (lib().bmb200_result_fetch_view_async, "result_fetch_view_async")
+        self.ctx.check(fn(self._h, C.byref(k), C.byref(o), C.byref(b), C.byref(g), C.byref(nb), C.byref(ng), C.byref(tot)), what)
+
+        def view(p, ctype, dtype, count):
+            if not count:
+                return np.empty(0, dtype)
+            a = np.ctypeslib.as_array(C.cast(p, C.POINTER(ctype)), shape=(count,))
+            return a.copy() if wait else a
+        return (view(k, C.c_uint8, np.uint8, self.n_cols), view(o, C.c_uint64, np.uint64, self.n_cols),
+                view(b, C.c_uint32, np.uint32, nb.value * BLOCK_WORDS), view(g, C.c_uint16, np.uint16, ng.value),
+                nb.value, ng.value, tot.value)
+
+    def fetch_wait(self, col: int):
+        """bmb200_result_fetch_wait: returns once the blocks of columns [0, col] of the last fetch_view(wait=False) have landed."""
+        self.ctx.check(lib().bmb200_result_fetch_wait(self._h, C.c_uint32(int(col))), "result_fetch_wait")
 
     def fetch_column(self, col: int):
         """bmb200_result_fetch_column -> (kind, bits[2048] | None, gap words | None) of ONE result column."""
