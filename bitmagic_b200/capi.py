@@ -47,6 +47,7 @@ SYMBOLS = [
     "bmb200_result_fetch_column", "bmb200_set_run_lists", "bmb200_set_bit_run_lists",
     "bmb200_rank_decompress", "bmb200_rank_compress", "bmb200_scan_str", "bmb200_set_packed_singles",
     "bmb200_set_run_list_unions", "bmb200_set_coverage", "bmb200_sv_mismatch", "bmb200_sv_first_mismatch",
+    "bmb200_remap",
 ]
 OP_SUB = 5
 COMM_ID_BYTES = 128
@@ -112,6 +113,12 @@ class MismatchArgsC(C.Structure):
         ("plane0_a", C.c_uint32), ("n_planes_a", C.c_uint32), ("plane0_b", C.c_uint32), ("n_planes_b", C.c_uint32),
         ("not_null_a", C.c_uint32), ("not_null_b", C.c_uint32), ("size_a", C.c_uint64), ("size_b", C.c_uint64),
         ("null_proc", C.c_uint32), ("flags", C.c_uint32), ("nb_from", C.c_uint32), ("nb_to", C.c_uint32),
+    ]
+
+
+class RemapArgsC(C.Structure):
+    _fields_ = [
+        ("plane0", C.c_uint32), ("n_planes", C.c_uint32), ("not_null", C.c_uint32), ("flags", C.c_uint32), ("id_max", C.c_uint64),
     ]
 
 
@@ -721,6 +728,17 @@ def rank_compress(ctx: Context, rs: "DeviceRS", src_vec: int, flags: int = 0, re
     NOT-NULL vector and packed to its ranks; one group of max(1, ceil(count / 65536)) columns."""
     out = result if result is not None else DeviceResult(ctx)
     ctx.check(lib().bmb200_rank_compress(ctx._h, rs._h, int(src_vec), int(flags), C.byref(out._h)), "rank_compress")
+    return _sized(out)
+
+
+def remap(ctx: Context, dset: DeviceSet, src: DeviceResult, plane0: int, n_planes: int, not_null: int = NO_UNIVERSE,
+          id_max: int = 0xFFFFFFFF, flags: int = 0, result: DeviceResult | None = None) -> DeviceResult:
+    """bmb200_remap (set2set_11_transform::remap): the values the set bits of `src` (one group; column c = element block c)
+    hold in the sparse vector whose plane j is set vector plane0 + j, inside its NOT-NULL vector `not_null` when it is
+    nullable; values >= id_max are left out.  One group of max(1, 2^(n_planes - 16)) columns."""
+    out = result if result is not None else DeviceResult(ctx)
+    args = RemapArgsC(int(plane0), int(n_planes), int(not_null), int(flags), int(id_max))
+    ctx.check(lib().bmb200_remap(ctx._h, dset._h, C.byref(args), src._h, C.byref(out._h)), "remap")
     return _sized(out)
 
 

@@ -16,6 +16,7 @@
 #include "mismatch_kernel.cuh"
 #include "str_scan_kernel.cuh"
 #include "rank_kernel.cuh"
+#include "remap_kernel.cuh"
 #include "shift_kernel.cuh"
 #include "binop_kernel.cuh"
 #include <algorithm>
@@ -43,7 +44,7 @@ enum DevSlot {
     kDevRsFound,                      //   select's found flags
     kDevSlabMirror,                   // bmb200_set_upload_slabs: the device mirror of the slabs (freed by bmb200_ctx_trim)
     kDevSlabSrc,                      //   where each block sits in the mirror (freed by bmb200_ctx_trim)
-    kDevRankDense,                    // bmb200_rank_compress: the dense scatter target
+    kDevDense,                        // bmb200_rank_compress, bmb200_remap: the dense scatter target
     kDevBlobStage,                    // bmb200_set_upload_blobs: the BLOB bytes
     kDevBlobOff, kDevBlobSize,        //   per-vector offset and size inside the staged bytes
     kDevBlobToks, kDevBlobNToks,      //   pass 1: token table, tokens per segment
@@ -2636,7 +2637,7 @@ int bmb200_rank_compress(bmb200_ctx* ctx, const bmb200_rs* idx, uint32_t src_vec
     const uint32_t cols = (uint32_t)cols64;
     const bool compress = (flags & BMB200_F_OPT_COMPRESS) != 0;
     uint32_t* dense = nullptr;
-    int rc = pool_dev(ctx, kDevRankDense, (size_t)cols * BMB200_BLOCK_BYTES, (void**)&dense);
+    int rc = pool_dev(ctx, kDevDense, (size_t)cols * BMB200_BLOCK_BYTES, (void**)&dense);
     if (rc) return rc;
     bmb200_result* r = nullptr;
     if ((rc = prepare_result(ctx, cols, 1u, true, compress, compress, kOrRefuse, inout, &r))) return rc;
@@ -2645,6 +2646,50 @@ int bmb200_rank_compress(bmb200_ctx* ctx, const bmb200_rs* idx, uint32_t src_vec
     if (e == cudaSuccess) e = cudaMemsetAsync(r->total, 0, 8, ctx->stream);
     if (e != cudaSuccess) { ctx->last_err = std::string("rank_compress: ") + cudaGetErrorString(e); return bail(r, inout, BMB200_ERR_CUDA); }
     rank_compress_scatter_kernel<<<work_grid(ctx, idx->n_blocks, kCtasPerSm), kAggThreads, 0, ctx->stream>>>(rs_view(idx), src_vec, dense);
+    if ((rc = after_launch(ctx))) return bail(r, inout, rc);
+    AggParams p{};
+    p.n_groups = 1; p.n_cols = cols; p.compress = compress ? 1u : 0u; p.store_blocks = 1u;
+    p.blocks = r->blocks; p.popcnt = r->popcnt; p.digest = r->digest; p.nruns = r->nruns; p.kind = r->kind; p.gaps = r->gaps;
+    p.total = r->total;
+    finalize_blocks_kernel<<<work_grid(ctx, cols, kCtasPerSm), kAggThreads, 0, ctx->stream>>>(p, dense);
+    return launch_epilogue(ctx, r, inout, false);
+}
+
+/* ------------------------------------------------------------------ set image through a sparse vector (remap_kernel.cuh) */
+
+int bmb200_remap(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_remap_args* a, const bmb200_result* src, bmb200_result** inout)
+{
+    if (!ctx || !set || !a || !src || !inout || set->ctx != ctx || src->ctx != ctx || *inout == src) return BMB200_ERR_BADARG;
+    if ((a->flags & ~BMB200_F_OPT_COMPRESS) || !a->n_planes) return BMB200_ERR_BADARG;
+    if (a->n_planes > 32u) return BMB200_ERR_RANGE;
+    if ((uint64_t)a->plane0 + a->n_planes > set->v.n_vec || (a->not_null != 0xffffffffu && a->not_null >= set->v.n_vec))
+        return BMB200_ERR_BADARG;
+    // the source's columns are read by their kind, as bmb200_rank_decompress reads them
+    if (!src->has_blocks || !src->blocks || src->n_groups != 1u || (src->compress && (!src->gaps || !src->gaps_ready)))
+        return BMB200_ERR_BADARG;
+    CU(cudaSetDevice(ctx->device));
+    const uint32_t cols = a->n_planes > 16u ? 1u << (a->n_planes - 16u) : 1u;    // the image holds every value below 2^n_planes
+    const bool compress = (a->flags & BMB200_F_OPT_COMPRESS) != 0;
+    uint32_t* dense = nullptr;
+    int rc = pool_dev(ctx, kDevDense, (size_t)cols * BMB200_BLOCK_BYTES, (void**)&dense);
+    if (rc) return rc;
+    bmb200_result* r = nullptr;
+    if ((rc = prepare_result(ctx, cols, 1u, true, compress, compress, kOrRefuse, inout, &r))) return rc;
+    r->gaps_ready = compress;                             // the epilogue writes the GAP form in compress mode
+    if (cudaMemsetAsync(dense, 0, (size_t)cols * BMB200_BLOCK_BYTES, ctx->stream) != cudaSuccess) {
+        ctx->last_err = "remap: memset"; return bail(r, inout, BMB200_ERR_CUDA);
+    }
+    if ((rc = launch_prologue(ctx, r, inout, 1u, "remap"))) return rc;
+    const size_t smem = remap_smem(a->n_planes);
+    if (cudaFuncSetAttribute(remap_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)remap_smem(32)) != cudaSuccess) {
+        ctx->last_err = "remap: cudaFuncSetAttribute"; return bail(r, inout, BMB200_ERR_CUDA);
+    }
+    RemapParams rp{};
+    rp.set = set->v;
+    rp.src = RankSrc{src->kind, src->blocks, src->gaps, src->cols_per_group};
+    rp.n_cols = src->n_cols; rp.plane0 = a->plane0; rp.n_planes = a->n_planes; rp.not_null = a->not_null;
+    rp.id_max = a->id_max; rp.dense = dense; rp.work_counter = ctx->d_work;
+    remap_kernel<<<work_grid(ctx, src->n_cols, kCtasPerSm), kAggThreads, smem, ctx->stream>>>(rp);
     if ((rc = after_launch(ctx))) return bail(r, inout, rc);
     AggParams p{};
     p.n_groups = 1; p.n_cols = cols; p.compress = compress ? 1u : 0u; p.store_blocks = 1u;

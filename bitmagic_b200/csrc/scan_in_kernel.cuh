@@ -91,6 +91,43 @@ __device__ __forceinline__ void gap_expand_chunk(uint32_t* row, const uint16_t* 
     }
 }
 
+// Stage words [c0, c0 + kInChunkWords) of the blocks desc(0..n_rows) of one column into the odd-stride rows: 16-byte loads of
+// the bit blocks (kInLoads in flight per thread), scalar stores; GAP rows start zeroed and get their runs ORed in (any_gap: some
+// desc(r) is GAP, the same for every thread).  Ends with a barrier, so the rows can be read.  scan_in_kernel and remap_kernel.
+template <class Desc>
+__device__ __forceinline__ void stage_chunk(uint32_t* rows, uint32_t n_rows, const Desc& desc, bool any_gap, const uint4* bseg,
+                                            const uint16_t* gseg, uint32_t c0, int tid)
+{
+    const uint32_t nq = n_rows * (kInChunkWords / 4u);
+    for (uint32_t q0 = tid; q0 < nq; q0 += kInLoads * kAggThreads) {
+        uint4 v[kInLoads];
+#pragma unroll
+        for (int u = 0; u < kInLoads; ++u) {
+            const uint32_t q = q0 + u * kAggThreads, r = q / (kInChunkWords / 4u);
+            const uint32_t d = q < nq ? desc(r) : BMB200_BLK_NULL, kind = d & 3u;
+            v[u] = make_uint4(0u, 0u, 0u, 0u);
+            if (kind == BMB200_BLK_BIT) v[u] = ld_stream_v4(bseg + (size_t)(d >> 2) * (kBlockWords / 4) + c0 / 4u + q % (kInChunkWords / 4u));
+            else if (kind == BMB200_BLK_FULL) v[u] = make_uint4(~0u, ~0u, ~0u, ~0u);
+        }
+#pragma unroll
+        for (int u = 0; u < kInLoads; ++u) {
+            const uint32_t q = q0 + u * kAggThreads;
+            if (q >= nq) break;
+            uint32_t* dst = rows + (q / (kInChunkWords / 4u)) * kInRowStride + 4u * (q % (kInChunkWords / 4u));
+            dst[0] = v[u].x; dst[1] = v[u].y; dst[2] = v[u].z; dst[3] = v[u].w;
+        }
+    }
+    if (any_gap) {
+        __syncthreads();
+        for (uint32_t r = 0; r < n_rows; ++r) {
+            const uint32_t d = desc(r);
+            if ((d & 3u) != BMB200_BLK_GAP) continue;
+            gap_expand_chunk(rows + r * kInRowStride, gap_block_ptr(gseg, d), 32u * c0, tid);
+        }
+    }
+    __syncthreads();
+}
+
 // WIDE: more than 32 planes (codes in two transposed halves)
 template <bool WIDE>
 __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_in_kernel(const ScanInParams sp)
@@ -127,37 +164,9 @@ __global__ void __launch_bounds__(kAggThreads, kCtasPerSm) scan_in_kernel(const 
         } else {
             bool any_gap = false;
             for (uint32_t r = 0; r <= np; ++r) any_gap |= ((r < np ? s_desc[r] : du) & 3u) == BMB200_BLK_GAP;
+            const auto desc = [&](uint32_t r) { return r < np ? s_desc[r] : du; };   // planes, then the universe
             for (uint32_t c0 = 0; c0 < kBlockWords; c0 += kInChunkWords) {
-                // stage the chunk: 16-byte loads of the bit planes (kInLoads in flight per thread), scalar stores into the
-                // odd-stride rows; GAP rows start zeroed
-                const uint32_t nq = (np + 1u) * (kInChunkWords / 4u);
-                for (uint32_t q0 = tid; q0 < nq; q0 += kInLoads * kAggThreads) {
-                    uint4 v[kInLoads];
-#pragma unroll
-                    for (int u = 0; u < kInLoads; ++u) {
-                        const uint32_t q = q0 + u * kAggThreads, r = q / (kInChunkWords / 4u);
-                        const uint32_t d = q < nq ? (r < np ? s_desc[r] : du) : BMB200_BLK_NULL, kind = d & 3u;
-                        v[u] = make_uint4(0u, 0u, 0u, 0u);
-                        if (kind == BMB200_BLK_BIT) v[u] = ld_stream_v4(bseg + (size_t)(d >> 2) * (kBlockWords / 4) + c0 / 4u + q % (kInChunkWords / 4u));
-                        else if (kind == BMB200_BLK_FULL) v[u] = make_uint4(~0u, ~0u, ~0u, ~0u);
-                    }
-#pragma unroll
-                    for (int u = 0; u < kInLoads; ++u) {
-                        const uint32_t q = q0 + u * kAggThreads;
-                        if (q >= nq) break;
-                        uint32_t* dst = rows + (q / (kInChunkWords / 4u)) * kInRowStride + 4u * (q % (kInChunkWords / 4u));
-                        dst[0] = v[u].x; dst[1] = v[u].y; dst[2] = v[u].z; dst[3] = v[u].w;
-                    }
-                }
-                if (any_gap) {                                                // uniform
-                    __syncthreads();
-                    for (uint32_t r = 0; r <= np; ++r) {
-                        const uint32_t d = r < np ? s_desc[r] : du;
-                        if ((d & 3u) != BMB200_BLK_GAP) continue;
-                        gap_expand_chunk(rows + r * kInRowStride, gap_block_ptr(gseg, d), 32u * c0, tid);
-                    }
-                }
-                __syncthreads();
+                stage_chunk(rows, np + 1u, desc, any_gap, bseg, gseg, c0, tid);
                 // one 32-element word per warp and step: transpose the planes into codes, look the codes inside U up
                 for (uint32_t w = (uint32_t)warp; w < kInChunkWords; w += kAggWarps) {
                     const uint32_t uw = rows[np * kInRowStride + w];

@@ -618,6 +618,105 @@ bool sparse_vector_find_first_mismatch(context& ctx, const SV& sv1, const SV& sv
     return found != 0;
 }
 
+// ---- set image through a sparse vector: set2set_11_transform, src/bmsparsevec_algo.h:1902-2205 ----
+namespace detail {
+
+/// the vectors the reference's remap compiles for: a plain sparse_vector whose value_type is its bvector's size_type
+template<class SV> struct remap_vector : std::false_type {};
+template<class T, class BV> struct remap_vector<bm::sparse_vector<T, BV>> : std::is_same<T, typename BV::size_type> {};
+
+} // namespace detail
+
+/// bm::set2set_11_transform<SV> on the device: attach_sv uploads the translation vector's trimmed planes and NOT-NULL vector
+/// once; every remap uploads bv_in as its own set and is one bmb200_remap launch (csrc/remap_kernel.cuh).  bv_out is replaced by
+/// the set of values sv[i] of the ids i of bv_in (inside the NOT-NULL vector of a nullable sv; a non-nullable sv maps ids without
+/// an element, and ids past its size(), to 0), without the value bm::id_max, as the reference computes it.  compute_stats
+/// changes the reference's work, not its answer, and is accepted and ignored.  Values of 2^32 and more are not covered:
+/// attach_sv throws std::length_error for a vector with more than 32 effective planes (BM64ADDR only).
+template<class SV>
+class set2set_11_transform
+{
+public:
+    typedef typename SV::bvector_type bvector_type;
+    typedef typename SV::value_type value_type;
+    typedef typename SV::size_type size_type;
+    static_assert(detail::remap_vector<SV>::value,
+                  "bm::b200::set2set_11_transform maps through bm::sparse_vector<bvector_type::size_type> only, as the reference");
+
+    explicit set2set_11_transform(context& c) : ctx_(c) {}
+    ~set2set_11_transform() { if (set_) bmb200_set_free(set_); }
+    set2set_11_transform(const set2set_11_transform&) = delete; set2set_11_transform& operator=(const set2set_11_transform&) = delete;
+
+    /// attach (upload) a translation vector, nullptr to detach
+    void attach_sv(const SV* sv_brel, bool compute_stats = false)
+    {
+        (void)compute_stats;
+        if (set_) { bmb200_set_free(set_); set_ = nullptr; }
+        attached_ = sv_brel != nullptr;
+        if (!sv_brel || (empty_ = sv_brel->empty())) return;
+        std::vector<const bvector_type*> vecs;
+        unsigned n = detail::mismatch_set<SV>::planes(*sv_brel, vecs);
+        if (n > 32u) throw std::length_error("bm::b200::set2set_11_transform: values of 2^32 and more are not covered");
+        static const bvector_type empty;
+        if (!n) { vecs.push_back(&empty); n = 1; }
+        args_ = bmb200_remap_args{0u, n, 0xffffffffu, BMB200_F_OPT_COMPRESS, uint64_t(bm::id_max)};
+        if (const bvector_type* nn = sv_brel->get_null_bvector()) { args_.not_null = (uint32_t)vecs.size(); vecs.push_back(nn); }
+        const uint32_t n_blocks = detail::column_count(std::max<uint64_t>(detail::size_blocks(sv_brel->size()), 1u),
+                                                       "bm::b200::set2set_11_transform");
+        std::vector<detail::tree_view<bvector_type>> views(vecs.size());
+        std::vector<bmb200_vec_blocks> vb(vecs.size());
+        for (size_t j = 0; j < vecs.size(); ++j) {
+            views[j].build(*vecs[j], n_blocks);
+            vb[j].n_blocks = n_blocks; vb[j].kind = views[j].kind.data(); vb[j].ptr = views[j].ptr.data();
+        }
+        check(bmb200_set_upload_vectors(ctx_.get(), (uint32_t)vecs.size(), n_blocks, vb.data(), &set_), "bmb200_set_upload_vectors");
+    }
+
+    /// bv_out = the image of bv_in through the attached vector
+    void remap(const bvector_type& bv_in, bvector_type& bv_out)
+    {
+        bv_out.clear(true);
+        if (!attached_ || empty_) return;
+        const uint32_t n_blocks = std::max<uint32_t>(detail::extent_of(bv_in), 1u);
+        detail::tree_view<bvector_type> view; view.build(bv_in, n_blocks);
+        bmb200_vec_blocks vb{n_blocks, view.kind.data(), view.ptr.data()};
+        bmb200_set* in = nullptr; bmb200_result *src = nullptr, *res = nullptr;
+        int rc = bmb200_set_upload_vectors(ctx_.get(), 1u, n_blocks, &vb, &in);
+        if (!rc) {
+            // bv_in enters as a result, the form bmb200_remap reads: a one-source OR copies it
+            const uint32_t zero = 0u;
+            bmb200_agg_args a{BMB200_OP_OR, BMB200_F_OPT_NONE, &zero, 1u, nullptr, 0u, 0u, 0u};
+            rc = bmb200_aggregate(ctx_.get(), in, &a, &src);
+        }
+        if (!rc) rc = bmb200_remap(ctx_.get(), set_, &args_, src, &res);
+        uint64_t total = 0, nb = 0, ng = 0;
+        const uint8_t* kind = nullptr; const uint64_t* off = nullptr; const uint32_t* bits = nullptr; const uint16_t* gaps = nullptr;
+        uint32_t n_cols = 0;
+        if (!rc) rc = bmb200_result_device_ptrs(res, nullptr, nullptr, nullptr, nullptr, &n_cols);
+        if (!rc) rc = bmb200_result_fetch_view(res, &kind, &off, &bits, &gaps, &nb, &ng, &total);
+        if (!rc) detail::store_result(bv_out, bv_out.size(), n_cols, kind, off, bits, gaps);
+        if (res) bmb200_result_free(res);
+        if (src) bmb200_result_free(src);
+        if (in) bmb200_set_free(in);
+        check(rc, "bm::b200::set2set_11_transform::remap");
+    }
+
+    /// attach sv_brel, remap, detach (the reference's remap(bv_in, sv_brel, bv_out))
+    void remap(const bvector_type& bv_in, const SV& sv_brel, bvector_type& bv_out)
+    {
+        attach_sv(&sv_brel);
+        remap(bv_in, bv_out);
+        attach_sv(nullptr);
+    }
+    void run(const bvector_type& bv_in, const SV& sv_brel, bvector_type& bv_out) { remap(bv_in, sv_brel, bv_out); }
+
+private:
+    context& ctx_;
+    bmb200_set* set_ = nullptr;
+    bmb200_remap_args args_{};
+    bool attached_ = false, empty_ = true;
+};
+
 }} // namespace bm::b200
 
 #endif

@@ -384,3 +384,50 @@ def find_first_mismatch(sv1: SparseVector, sv2: SparseVector, use_null: bool = T
         return capi.sv_first_mismatch(ctx, dset, args)
     finally:
         dset.free()
+
+
+class Set2SetTransform:
+    """``bm::set2set_11_transform<sparse_vector<unsigned>>`` with the vector attached once (``attach_sv``): its planes and
+    NOT-NULL vector are uploaded at construction, and every ``remap(src)`` is one ``bmb200_remap`` launch
+    (csrc/remap_kernel.cuh).  ``src`` is a ``BVector`` (uploaded for the call) or a one-group ``DeviceResult`` (a scan or
+    aggregation result, read where it lies); the image comes back as a ``BVector``: the values ``sv[i]`` of the ids i of
+    ``src`` (inside the NOT-NULL vector of a nullable vector; ids without an element, or past ``size``, of a non-nullable
+    vector map to 0).  The value 0xFFFFFFFF (``bm::id_max`` of the 32-bit build) is left out, as the reference leaves it out."""
+
+    ID_MAX = 0xFFFFFFFF
+
+    def __init__(self, sv: SparseVector, ctx: capi.Context | None = None):
+        if type(sv) is not SparseVector or sv.signed:
+            raise TypeError("set2set_11_transform maps through an unsigned plain SparseVector (not signed, RSC, float or string)")
+        if len(sv.planes) > 32:
+            raise ValueError("values of a remap translation vector must fit 32 bits")
+        self.ctx = ctx or capi.default_context()
+        self.sv = sv
+        vecs = list(sv.planes) + ([sv.not_null] if sv.not_null is not None else [])
+        self._not_null = len(sv.planes) if sv.not_null is not None else capi.NO_UNIVERSE
+        self._dset = capi.DeviceSet.upload(self.ctx, PackedSet.pack(vecs, max(v.n_blocks for v in vecs)))
+
+    def close(self):
+        if self._dset is not None:
+            self._dset.free()
+            self._dset = None
+
+    def remap(self, src: BVector | capi.DeviceResult) -> BVector:
+        if self.sv.size == 0:                                  # an empty vector has an empty image
+            return BVector(1)
+        own, dset = None, None
+        try:
+            if isinstance(src, BVector):
+                # the input enters as a result, the form bmb200_remap reads: a one-source OR copies it
+                dset = capi.DeviceSet.upload(self.ctx, PackedSet.pack([src]))
+                own = src = capi.aggregate(self.ctx, dset, capi.OP_OR, [0])
+            res = capi.remap(self.ctx, self._dset, src, 0, len(self.sv.planes), self._not_null, self.ID_MAX, F_OPT_COMPRESS)
+            try:
+                return result_to_bvector(*res.fetch())
+            finally:
+                res.free()
+        finally:
+            if own is not None:
+                own.free()
+            if dset is not None:
+                dset.free()

@@ -37,6 +37,7 @@
  *   bmb200_rank_decompress        <- rank_compressor::decompress   src/bmalgo.h:571-644,
  *                                    sparse_vector_scanner::decompress src/bmsparsevec_algo.h:4525-4537
  *   bmb200_rank_compress          <- rank_compressor::compress     src/bmalgo.h:498-566
+ *   bmb200_remap                  <- set2set_11_transform::remap(bv_in, sv, bv_out)  src/bmsparsevec_algo.h:2097-2205
  *
  * Block geometry (src/bmconst.h:55-68,78-87): a bit-block is 2048 x u32 =
  * 8192 B = 65536 bits; a GAP block is u16 buf[0..len], buf[0] = header
@@ -545,6 +546,29 @@ int bmb200_rank_decompress(bmb200_ctx* ctx, const bmb200_rs* idx, const bmb200_r
  * bit of NN.  For src not a subset of NN the result is compress(src & NN); the reference requires src to be a subset
  * (src/bmalgo.h:526-549, asserted only) and computes an unspecified result otherwise. */
 int bmb200_rank_compress(bmb200_ctx* ctx, const bmb200_rs* idx, uint32_t src_vec, uint32_t flags, bmb200_result** inout);
+
+/* ---------------- set image through a sparse vector (set2set_11_transform::remap) ----------------
+ * set2set_11_transform<SV>::remap(bv_in, sv, bv_out) (src/bmsparsevec_algo.h:2097-2205) over a plain sparse vector whose
+ * value_type is the caller's bvector size_type: the set of values the ids of bv_in hold (SQL SELECT DISTINCT f(id)).
+ * code(i) = SUM_j plane_j[i] << j with plane j = set vector plane0 + j, planes read as 0 past the set's columns.  src is any
+ * result of one group with stored blocks; its column c is element block c (as bmb200_rank_decompress reads it).
+ * Out: one group of max(1, 2^(n_planes - 16)) columns.  Bit v is set iff v < id_max and some set bit i of src (inside the
+ * NOT-NULL vector when not_null != 0xffffffff) has code(i) = v.  A non-nullable vector maps ids without an assigned element,
+ * and ids at or past its size(), to 0.  id_max is bm::id_max of the caller's build: the reference leaves the value id_max
+ * out of its image (0xffffffff in the 32-bit build, 2^48 - 1 under BM64ADDR).  An empty vector (size() == 0) has an empty
+ * image: the caller clears its output without a launch.  Results are recycled through inout as usual; the count is
+ * bmb200_result_total / bmb200_result_group_totals.
+ * BMB200_ERR_BADARG for null pointers, a foreign context, src == *inout, a src without stored blocks or with more than one
+ * group, flags other than BMB200_F_OPT_NONE / BMB200_F_OPT_COMPRESS, n_planes == 0, plane or NOT-NULL ids outside the set;
+ * BMB200_ERR_RANGE for n_planes > 32 (images of values >= 2^32 are not covered). */
+typedef struct bmb200_remap_args {
+    uint32_t plane0, n_planes;   /* plane j of the translation vector = set vector plane0 + j; n_planes 1..32 */
+    uint32_t not_null;           /* its NOT-NULL vector; 0xffffffff = not nullable                              */
+    uint32_t flags;              /* BMB200_F_OPT_NONE / BMB200_F_OPT_COMPRESS                                   */
+    uint64_t id_max;             /* codes >= id_max are left out (bm::id_max of the caller's build)             */
+} bmb200_remap_args;
+int bmb200_remap(bmb200_ctx* ctx, const bmb200_set* set, const bmb200_remap_args* args,
+                 const bmb200_result* src, bmb200_result** inout);
 
 #ifdef __cplusplus
 }
